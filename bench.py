@@ -2,7 +2,8 @@
 """DDIM-100 autoencoding throughput (BASELINE.json metric) for the pdae_b200 hot path.
 
   python bench.py [--gpus N] [--steps K] [--warmup W]            # our CUDA path, one process per GPU (torchrun for N>1)
-  python bench.py --impl reference [...]                          # the UNMODIFIED reference (baseline/_ref) on the host CPU cores
+  python bench.py --impl reference [...]                          # the UNMODIFIED reference (oracle/_ref) on the host CPU cores
+  python bench.py --dump-outputs DIR [...]                        # also write the last timed step's reconstructions as DIR/*.npy
 
 One "step" = one full autoencoding pass over one synthetic batch: 1 semantic-encoder forward + S DDIM-encode steps + S
 DDIM-decode steps of the ShiftUNet (S=100 -> 200 decoder forwards + 200 fused DDIM updates).  `value` = images/s with
@@ -18,10 +19,12 @@ briefly and reported under `modes`.  Rank 0 prints ONE JSON line.
 import argparse
 import json
 import os
+import signal
 import subprocess
 import sys
 import threading
 import time
+import traceback
 
 ROOT = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, ROOT)
@@ -39,10 +42,25 @@ WORKLOADS = {
     "ffhq256": (FFHQ256_PROXY, 256, "ffhq128", 128, 8, 967.20),
 }
 ENC_GFLOP = {"celeba64": 0.134, "ffhq128": 0.616}
-REF_DIR = os.path.join(ROOT, "baseline", "_ref")
+REF_DIR = os.path.join(ROOT, "oracle", "_ref")
 GATE = 1e-5          # |recon-MSE(ours) - recon-MSE(reference)| on [0,1]-scaled images (metric/utils.py:62-63)
 MODE_ORDER = ("bf16", "bf16x3", "fp32")     # fastest first
-DTYPE = {"bf16": "bf16", "bf16x3": "bf16x3 (split-operand bf16 tcgen05 MMAs, fp32 accumulate: fp32-grade products)", "fp32": "f32"}
+METRIC = "ddim100_autoencoding_images_per_sec"
+_T0 = time.time()
+_PHASE = ["start"]
+
+
+def phase(name):
+    """Progress on stderr (stdout carries only the result line), so a run that is stopped shows how far it got."""
+    _PHASE[0] = name
+    print(f"[bench] {time.time() - _T0:7.1f} s  {name}", file=sys.stderr, flush=True)
+
+
+def failure_line(msg):
+    """The result line of a run that cannot produce a value: the error and the phase it was in."""
+    print(json.dumps({"metric": METRIC, "value": None, "unit": "images/s", "error": msg[-3000:], "phase": _PHASE[0],
+                      "elapsed_s": round(time.time() - _T0, 1)}), flush=True)
+DTYPE = {"bf16": "bf16", "bf16x3": "bf16x3 (split-operand bf16 wgmma, fp32 accumulate: fp32-grade products)", "fp32": "f32"}
 
 
 def parse():
@@ -60,11 +78,13 @@ def parse():
     ap.add_argument("--no-cpu-baseline", action="store_true")
     ap.add_argument("--no-profile", action="store_true")
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary-mode timing and the ffhq256 strong-scaling line")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps, write what the last timed step computed (rank 0) as DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
 class ClockSampler:
-    """nvidia-smi clocks / throttle reasons sampled DURING the timed region (B200_PROFILING.md)."""
+    """nvidia-smi clocks / throttle reasons sampled DURING the timed region."""
     Q = "clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown," \
         "clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
 
@@ -106,7 +126,7 @@ def peaks():
     if os.path.exists(p):
         d = json.load(open(p))
         return d.get("bf16_tflops_sustained", 1427.1), d.get("hbm_gbs", 6575.1), "measured (MEASURED_PEAKS.json, sustained bf16)"
-    return 1400.0, 6650.0, "fallback (B200_PROFILING.md)"
+    return 989.4, 3350.0, "data sheet (H100 SXM, 700 W: dense bf16, HBM3)"
 
 
 # ----------------------------------------------------------------------------------------------------------------------
@@ -162,8 +182,8 @@ def cpu_sample_port(dec, enc, c, size, enc_kind, enc_size, S, batch, n_steps, wa
 
 
 class ReferenceCPU:
-    """The UNMODIFIED reference (ckczzj/PDAE, vendored by __graft_entry__.build() into baseline/_ref -- git-ignored, travels
-    to the GPU box) driven through its own public API on the host CPU cores: model.shift_unet.ShiftUNet, the encoder
+    """The UNMODIFIED reference (ckczzj/PDAE, installed by __graft_entry__.build() into oracle/_ref when its sources are
+    available -- git-ignored) driven through its own public API on the host CPU cores: model.shift_unet.ShiftUNet, the encoder
     class, diffusion.ddim.DDIM.shift_ddim_sample.  None of this package's kernels or modules are on this path; only the
     synthetic state_dict is shared."""
 
@@ -231,10 +251,10 @@ def run_reference(args):
             vals.append((ips, t_step))
     ips = sum(v[0] for v in vals) / len(vals)
     ms = 1e3 * sum(v[1] for v in vals) / len(vals)
-    what = "unmodified reference modules (baseline/_ref: model.shift_unet.ShiftUNet + diffusion.ddim.DDIM.shift_ddim_sample, torch CPU fp32)" \
-        if kind == "reference" else "oracle port (baseline/_ref absent)"
+    what = "unmodified reference modules (oracle/_ref: model.shift_unet.ShiftUNet + diffusion.ddim.DDIM.shift_ddim_sample, torch CPU fp32)" \
+        if kind == "reference" else "oracle port (oracle/_ref absent)"
     sample = f"{what}; {b} images x 1 ShiftUNet DDIM step per bench step ({ms / 1e3:.2f} s), extrapolated to {2 * S} steps + 1 encoder forward per image"
-    line = {"impl": "reference", "metric": "ddim100_autoencoding_images_per_sec", "value": ips, "unit": "images/s",
+    line = {"impl": "reference", "metric": METRIC, "value": ips, "unit": "images/s",
             "n_gpus": args.gpus, "steps": args.steps, "warmup": args.warmup, "ms_per_step": ms, "higher_is_better": True,
             "scaling": "weak", "vs_baseline": None, "dtype": "f32", "data": "synthetic",
             "config": {"workload": f"{args.workload}-proxy ShiftUNet+encoder, DDIM-{S} encode + DDIM-{S} decode", "batch": b,
@@ -292,8 +312,13 @@ def main():
     world = int(os.environ.get("WORLD_SIZE", "1"))
     rank = int(os.environ.get("RANK", "0"))
     local = int(os.environ.get("LOCAL_RANK", "0"))
+    from pdae_b200.utils.host import host_cores
+    torch.set_num_threads(host_cores())   # the host-side legs below never run more threads than the CPUs granted
+    phase("device")
     dev = torch.device("cuda", local)
     torch.cuda.set_device(dev)
+    from pdae_b200 import _native
+    _native.require_device()   # load the kernels and check the device before the host-side work below
     dist = None
     if world > 1:
         import torch.distributed as dist
@@ -315,6 +340,7 @@ def main():
         return x if enc_size == size else torch.nn.functional.avg_pool2d(x, size // enc_size)
 
     # ---- parity gate (rank 0) and mode selection ---------------------------------------------------------------------
+    phase("parity gate")
     gate = None
     chosen = args.precision
     if args.precision == "auto":
@@ -359,11 +385,20 @@ def main():
             dist.barrier()
         return float(ms.item())
 
-    W = max(args.warmup, 3)
+    W = max(args.warmup, 1)   # one pass records every plan and CUDA graph of the timed path
+    phase(f"warm-up ({chosen}, {W} pass(es))")
     for _ in range(W):
         autoencode(x_dev)
+    last = {}
+
+    def step():
+        last["reconstruction"] = autoencode(x_dev)
+
+    phase(f"timed steps ({args.steps})")
     with ClockSampler(local) as clk:
-        ms_total = timed(lambda: autoencode(x_dev), args.steps)
+        ms_total = timed(step, args.steps)
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, last)
     ms_step = ms_total / args.steps
     value = world * B / (ms_step / 1e3)
 
@@ -372,8 +407,8 @@ def main():
         rec = autoencode(xd)
         out_host.copy_(rec, non_blocking=True)
 
-    e2e_steps = max(1, min(args.steps, 3))     # (a full pass each; bounded so the default run stays within minutes)
-    e2e_once()
+    phase("end-to-end pass")
+    e2e_steps = 1     # one full pass; the plans and graphs are already warm from the timed steps
     ms_e2e = timed(e2e_once, e2e_steps) / e2e_steps
     e2e_val = world * B / (ms_e2e / 1e3)
 
@@ -415,12 +450,14 @@ def main():
                 roof["traffic_unit"] = "bytes/launch (ncu dram__bytes_read.sum + dram__bytes_write.sum, profiles/conv_traffic.json)"
         return roof, kinds
 
+    phase("kernel view")
     roof, kinds = (None, {}) if args.no_profile else kernel_view(plan)
 
     # ---- extras: the other tensor-core mode, and the FFHQ-256 strong-scaling configuration ---------------------------------
     modes = {}
     extras = {}
     if not args.no_extras:
+        phase("extras")
         other = [m for m in ("bf16", "bf16x3") if m != chosen]
         for m in other:
             try:
@@ -453,7 +490,7 @@ def main():
 
     flop_img = (2 * S * gflop_step + ENC_GFLOP[enc_kind]) * 1e9
     line = {
-        "metric": "ddim100_autoencoding_images_per_sec", "value": round(value, 4), "unit": "images/s", "n_gpus": world,
+        "metric": METRIC, "value": round(value, 4), "unit": "images/s", "n_gpus": world,
         "steps": args.steps, "warmup": W, "ms_per_step": round(ms_step, 3), "higher_is_better": True,
         "scaling": "weak", "vs_baseline": None, "dtype": DTYPE[chosen], "data": "synthetic",
         "config": {"workload": f"{args.workload}-proxy ShiftUNet+encoder (proxy decoder config, SURVEY D4), {size}x{size}x3, "
@@ -471,13 +508,14 @@ def main():
         "roofline": roof, "kernels_per_decoder_step": kinds, "modes": modes, "extras": extras,
     }
     if not args.no_cpu_baseline and world == 1:   # the CPU baseline is an N=1, rank-0 leg
+        phase("cpu baseline")
         b = cpu_batch(size)
         if have_reference():
             ips, cores, t_step, t_enc = ReferenceCPU(dec_cpu, enc_cpu, c, enc_kind, S).sample(size, enc_size, S, b, n_steps=3)
-            kind, what = "reference", "unmodified reference modules from baseline/_ref (torch CPU fp32)"
+            kind, what = "reference", "unmodified reference modules from oracle/_ref (torch CPU fp32)"
         else:
             ips, cores, t_step, t_enc = cpu_sample_port(dec_cpu, enc_cpu, c, size, enc_kind, enc_size, S, b, n_steps=3)
-            kind, what = "port", "oracle (torch-CPU restatement of the reference; baseline/_ref absent)"
+            kind, what = "port", "oracle (torch-CPU restatement of the reference; oracle/_ref absent)"
         line["cpu_baseline"] = {"value": ips, "unit": "images/s", "cores": cores, "kind": kind,
                                 "sample": f"{what}, batch {b}: 1 warm-up + 3 timed ShiftUNet DDIM steps ({t_step:.2f} s/step) + 1 "
                                           f"encoder forward, extrapolated to {2 * S} steps per image"}
@@ -486,6 +524,21 @@ def main():
     print(json.dumps(line))
     if world > 1:
         dist.destroy_process_group()
+
+
+def dump_outputs(path, arrays, limit=64 << 20):
+    """Write each array as <path>/<name>.npy in float32, at most `limit` bytes in all: an array that does not fit is replaced by
+    a fixed, seeded sample of its elements (flattened), so two builds given the same arguments can be compared output for
+    output."""
+    import numpy as np
+    os.makedirs(path, exist_ok=True)
+    budget = limit // max(1, len(arrays))
+    for name, t in arrays.items():
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes > budget:
+            idx = np.sort(np.random.default_rng(0).choice(a.size, budget // 4, replace=False))
+            a = a.reshape(-1)[idx]
+        np.save(os.path.join(path, f"{name}.npy"), a)
 
 
 def strong_scaling_extra(gd, precision, world, rank, dev, timed):
@@ -528,7 +581,7 @@ def strong_scaling_extra(gd, precision, world, rank, dev, timed):
 
 
 def reference_gpu_extra(dec_cpu, enc_cpu, c, enc_kind, S, B, size, enc_size, dev, enc_input):
-    """Context, not the contract's reference arm (that one is the CPU run): the UNMODIFIED reference modules (baseline/_ref) on
+    """Context, not the reference arm (that one is the CPU run): the UNMODIFIED reference modules (oracle/_ref) on
     THIS GPU through stock PyTorch -- eager mode, fp32 parameters, TF32 convolutions / matmuls as the reference's trainers set
     (trainer/base_trainer.py:24-25).  (1) images/s of the same workload from timed DDIM steps; (2) the same 1e-5 gate probe:
     does the reference's own GPU arithmetic reproduce its CPU fp32 result on these weights?"""
@@ -661,5 +714,15 @@ def training_step_extra(world, rank, dev, timed):
         return {"error": repr(e)[:300]}
 
 
+def _terminated(signum, frame):
+    failure_line(f"terminated by signal {signum}")
+    sys.exit(128 + signum)
+
+
 if __name__ == "__main__":
-    main()
+    signal.signal(signal.SIGTERM, _terminated)
+    try:
+        main()
+    except Exception:
+        failure_line(traceback.format_exc())
+        raise

@@ -1,9 +1,9 @@
-/* pdae_b200 -- C-ABI of the B200-native PDAE hot path (libpdae_b200.so).
+/* pdae_b200 -- C-ABI of the Hopper-native (H100) PDAE hot path (libpdae_b200.so).
  *
  * The reference (ckczzj/PDAE) has no FFI: its hot path is PyTorch ATen dispatches issued from
  * model/module.py, model/unet.py, model/shift_unet.py, diffusion/ddim.py and
  * diffusion/gaussian_diffusion.py.  Each entry point below replaces the ATen call group named in
- * its comment (reference file:line) with one hand-written sm_100a kernel launch.
+ * its comment (reference file:line) with one hand-written sm_90a kernel launch.
  *
  * Conventions
  *   - plain pointers and sizes only; every pointer is DEVICE memory owned by the caller;
@@ -12,7 +12,7 @@
  *     inside CUDA-graph capture;
  *   - return 0 on success, a negative PDAE_E* code otherwise; pdae_last_error() gives the message
  *     (thread-local).  Nothing throws or aborts.
- *   - there is NO CPU fallback: without an sm_100 device every compute entry point fails.
+ *   - there is NO CPU fallback: without an sm_90 device every compute entry point fails.
  */
 #ifndef PDAE_B200_H
 #define PDAE_B200_H
@@ -28,7 +28,7 @@ typedef void* pdae_stream_t; /* cudaStream_t */
 #define PDAE_OK 0
 #define PDAE_EINVAL (-1)  /* bad argument / unsupported shape */
 #define PDAE_ECUDA (-2)   /* CUDA runtime / launch error      */
-#define PDAE_ENODEV (-3)  /* no sm_100 device                 */
+#define PDAE_ENODEV (-3)  /* no sm_90 device                  */
 
 #define PDAE_F32 0
 #define PDAE_BF16 1
@@ -39,7 +39,7 @@ typedef void* pdae_stream_t; /* cudaStream_t */
 
 const char* pdae_last_error(void);
 int pdae_abi_version(void);
-/* 0 if the current device is sm_100 (B200), PDAE_ENODEV otherwise. */
+/* 0 if the current device is sm_90 (H100), PDAE_ENODEV otherwise. */
 int pdae_device_check(void);
 
 /* ---- implicit-GEMM convolution / linear, fp32 CUDA-core math ("parity mode") -------------------
@@ -147,7 +147,7 @@ int pdae_mlp_mod_ln_act(const float* h, const float* cond, const float* ln_w, co
 /* dst[b][col0 + j] = src[b][j], j < N (row strides dst_ld / N).                                       */
 int pdae_copy_cols(const float* src, float* dst, int dst_ld, int col0, int B, int N, pdae_stream_t stream);
 
-/* ---- tensor-core convolution: TMA -> tcgen05.mma (bf16 x bf16 -> fp32 in TMEM) ---------------------
+/* ---- tensor-core convolution: TMA -> wgmma (bf16 x bf16 -> fp32 in registers) ---------------------
  * Same contract as pdae_conv2d_simt for ksize in {1,3}, stride 1, pad ksize/2, Cin % 64 == 0,
  * Cout % 64 == 0, bf16 NHWC input (already normalised/activated by pdae_gn_apply), weights bf16
  * [k*k][Cout][Cin].  A plan owns the TMA descriptors for fixed buffers; run it any number of times.   */
@@ -219,7 +219,7 @@ void pdae_conv_tc3_destroy(pdae_conv_tc3_plan* plan);
  * under trainer/train_representation_learning.py:112 loss.backward(); convs of model/module.py:241-259, 278-297):
  * dw[tap][cin][cout] += sum_{b,y,x} act[b, y+dy, x+dx, cin] * dy[b, y, x, cout].  act3 / dy3: bf16 NHWC with 3*C channels,
  * split-operand blocks [hi | lo | hi] (pdae_gn_apply_split3); every product is a_hi*d_hi + a_lo*d_hi + a_hi*d_lo with fp32
- * accumulation in TMEM (fp32-grade).  dw must be zeroed by the caller (split-K partial sums are added with fp32 reductions).
+ * accumulation in registers (fp32-grade).  dw must be zeroed by the caller (split-K partial sums are added with fp32 reductions).
  * Shapes: Cin % 64 == 0, Cout % 64 == 0, images tileable by 64-pixel TMA boxes (pdae_wgrad_tc_supported). */
 typedef struct pdae_wgrad_tc_plan pdae_wgrad_tc_plan;
 int pdae_wgrad_tc_supported(int H, int W, int Cin, int Cout, int ksize);
@@ -228,7 +228,7 @@ int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan, const void* act3_bf16, const
 int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* plan, pdae_stream_t stream);
 void pdae_wgrad_tc_destroy(pdae_wgrad_tc_plan* plan);
 
-/* v2: persistent CTAs, double-buffered TMEM accumulators (epilogue overlaps the next tile's main loop), TMA-store
+/* v2: persistent CTAs, two consumer warpgroups with register accumulators (the producer runs ahead into the next tile), TMA-store
  * epilogue.  out_dtype PDAE_F32|PDAE_BF16; ch_stats (optional) fp32 [B][Cout][2] accumulates per-channel (sum, sum^2)
  * of the stored values (zero it first); a residual is read in the OUTPUT's dtype.  cout_valid > 0 selects the image-head variant:
  * Cout must be 16 (weights zero-padded), `out` is NCHW fp32 [B][cout_valid][H][W].  bn_override: 0 = auto.              */
@@ -254,7 +254,7 @@ int pdae_gemm_tc2_create(pdae_conv_tc2_plan** plan, const void* a_bf16, long lon
                          long long b_ld, long long b_bs, void* out, int out_dtype, long long out_ld, long long out_bs,
                          int batch, int M, int N, int K);
 /* P_i = softmax_rows(alpha * A_i * Bm_i^T) stored as bf16 (ld / batch strides as above): attention probabilities with the
- * softmax (module.py:455, :486) folded into the GEMM epilogue -- the fp32 scores never leave TMEM.  N in {64,128,256}.     */
+ * softmax (module.py:455, :486) folded into the GEMM epilogue -- the fp32 scores never leave the registers.  N in {64,128,256}.     */
 int pdae_gemm_tc2_softmax_create(pdae_conv_tc2_plan** plan, const void* a_bf16, long long a_ld, long long a_bs,
                                  const void* b_bf16, long long b_ld, long long b_bs, void* out_bf16, long long out_ld,
                                  long long out_bs, int batch, int M, int N, int K, float alpha);
@@ -268,7 +268,7 @@ int pdae_softmax_bf16(const float* S, void* P_bf16, int64_t rows, int cols, floa
 int pdae_transpose_v(const void* qkv_bf16, void* vT_bf16, int B, int T, int C, int heads, int legacy, pdae_stream_t stream);
 /* Split-operand ("bf16x3") attention: re-lay the fp32 qkv rows as bf16 blocks Q3 = [q_hi|q_lo|q_hi], K3 = [k_hi|k_hi|k_lo]
  * ([B*heads][T][3*ch]) and VT3 = [vT_hi|vT_hi|vT_lo] ([B*heads][ch][3*T]) so that QK^T and PV (model/module.py:452-456,
- * 483-487) run as batched tcgen05 GEMMs with fp32-grade products; pdae_softmax_split3 turns the fp32 scores into
+ * 483-487) run as batched wgmma GEMMs with fp32-grade products; pdae_softmax_split3 turns the fp32 scores into
  * P3 = [p_hi|p_lo|p_hi] with p = softmax(alpha * S) evaluated in fp32.                                                  */
 int pdae_qkv_split3(const float* qkv, void* Q3, void* K3, void* VT3, int B, int T, int C, int heads, int legacy,
                     pdae_stream_t stream);

@@ -7,8 +7,8 @@ it follows.  Nothing here is imported by ``pdae_b200`` (the product); only
 ``tests/``, ``__graft_entry__.smoke()`` and ``bench.py``'s CPU-baseline /
 ``--impl reference`` legs may import this module.
 
-Parity status: PINNED.  ``tests/golden/make_golden.py`` (run in the build
-container, where ``/root/reference`` is importable) drives the *real* reference
+Parity status: PINNED.  ``tests/golden/make_golden.py`` (run where the
+reference sources are importable) drives the *real* reference
 modules on seeded inputs + deterministic weights and commits the outputs under
 ``tests/golden/*.npz``; ``tests/test_oracle_golden.py`` checks this file
 against every one of them (CPU, no GPU needed).  The reference itself ships no

@@ -1,4 +1,4 @@
-"""pdae_b200 -- B200-native (sm_100a) implementation of the PDAE hot path.
+"""pdae_b200 -- Hopper-native (H100, sm_90a) implementation of the PDAE hot path.
 
 Public surface mirrors the reference repo's modules:
     pdae_b200.model.unet.UNet, pdae_b200.model.shift_unet.ShiftUNet, pdae_b200.model.mlp_skip_net.MLPSkipNet,

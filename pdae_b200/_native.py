@@ -1,9 +1,8 @@
 """Build + ctypes binding of libpdae_b200.so (the C-ABI in include/pdae_b200.h).
 
 The library is built in-tree by ``build()`` (called from ``__graft_entry__.build()``) with
-``nvcc -gencode arch=compute_100a,code=sm_100a`` so the .so travels with the repo snapshot.  There is
-no CPU fallback anywhere in this package: if the library is missing or the device is not sm_100,
-every compute path raises.
+``nvcc -gencode arch=compute_90a,code=sm_90a`` (Hopper, H100).  There is no CPU fallback anywhere in
+this package: if the library is missing or the device is not sm_90, every compute path raises.
 """
 from __future__ import annotations
 
@@ -29,14 +28,15 @@ class NativeError(RuntimeError):
 
 
 def build(force: bool = False, verbose: bool = False) -> str:
-    """Compile every CUDA source for sm_100a into pdae_b200/libpdae_b200.so (cross-compiles without a GPU)."""
+    """Compile every CUDA source for sm_90a into pdae_b200/libpdae_b200.so (cross-compiles without a GPU)."""
     srcs = [os.path.join(_HERE, "csrc", s) for s in SOURCES]
-    deps = srcs + [os.path.join(_HERE, "csrc", "common.cuh"), os.path.join(_HERE, "csrc", "plan_exec_table.inc"),
+    deps = srcs + [os.path.join(_HERE, "csrc", "common.cuh"), os.path.join(_HERE, "csrc", "wgmma.cuh"),
+                   os.path.join(_HERE, "csrc", "plan_exec_table.inc"),
                    os.path.join(_ROOT, "include", "pdae_b200.h")]
     if not force and os.path.exists(LIB_PATH) and all(os.path.getmtime(LIB_PATH) >= os.path.getmtime(d) for d in deps):
         return LIB_PATH
     nvcc = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-    cmd = [nvcc, "-gencode", "arch=compute_100a,code=sm_100a", "-lineinfo", "-O3", "-std=c++17",
+    cmd = [nvcc, "-gencode", "arch=compute_90a,code=sm_90a", "-lineinfo", "-O3", "-std=c++17",
            "-I", os.path.join(_ROOT, "include"), "-I", os.path.join(_HERE, "csrc"),
            "-shared", "-Xcompiler", "-fPIC", "-o", LIB_PATH] + srcs
     if verbose:

@@ -3,7 +3,7 @@
 // GEMM view: M = B*Ho*Wo output pixels, N = Cout, K = k*k*Cin (tap-major, channel-minor so that
 // consecutive k are consecutive NHWC channels).  64x64x16 CTA tile, 256 threads, 4x4 micro-tile.
 // This is the exact-fp32 path used (a) to hold rtol 1e-3 / atol 1e-4 against the CPU oracle and
-// (b) for the shapes the tcgen05 kernel does not take (Cin=3 stem, stride-2 encoder convs, Linear).
+// (b) for the shapes the tensor-core kernels do not take (Cin=3 stem, stride-2 encoder convs, Linear).
 #include "common.cuh"
 
 namespace pdae {

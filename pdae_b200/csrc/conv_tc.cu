@@ -1,19 +1,20 @@
-// Tensor-core implicit-GEMM convolution for sm_100a:  TMA (im2col-free, OOB zero fill = conv padding)
-//   -> 128B-swizzled shared-memory stages -> tcgen05.mma (bf16 x bf16 -> fp32 accumulators in TMEM)
-//   -> tcgen05.ld epilogue (+bias, +residual) -> fp32 NHWC.
+// Tensor-core implicit-GEMM convolution for sm_90a:  TMA (im2col-free, OOB zero fill = conv padding)
+//   -> 128B-swizzled shared-memory stages -> wgmma (bf16 x bf16 -> fp32 accumulators in registers)
+//   -> epilogue (+bias, +residual) -> fp32 NHWC.
 //
 // GEMM view per CTA: D[128 pixels][BN couts] = sum over (tap, 64-channel block) of
 //     A_tap[128 pixels][64 ch] * W_tap[BN couts][64 ch]^T
 // The 128-pixel M tile is a (tn images) x (th rows) x (tw cols) box of the NHWC activation, fetched by
 // ONE 4-D TMA per (tap, channel block) at coordinates shifted by the tap offset; out-of-image
 // coordinates are zero-filled by the TMA unit, which is exactly the conv's zero padding.  Both operands
-// land K-major with the 128-byte swizzle, i.e. the canonical UMMA SW128 layout (8-row atoms of 1024 B).
+// land K-major with the 128-byte swizzle, i.e. the canonical wgmma SW128 layout (8-row atoms of 1024 B).
 //
-// Warp roles (192 threads): warp 0 = TMA producer, warp 1 = TMEM allocator + MMA issuer,
-// warps 2..5 = epilogue (warp%4 selects the 32-lane TMEM quadrant it may read).
+// Warp roles (288 threads): warps 0-7 = two consumer warpgroups (tile rows 0-63 / 64-127: wgmma + epilogue),
+// warp 8 = TMA producer.
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pdae {
 
@@ -21,7 +22,7 @@ constexpr int TC_BM = 128;
 constexpr int TC_BK = 64;                         // bf16 elements = 128 bytes = one swizzle row
 constexpr int TC_A_BYTES = TC_BM * TC_BK * 2;     // 16 KB
 constexpr int TC_MAX_STAGES = 8;
-constexpr int TC_THREADS = 192;
+constexpr int TC_THREADS = 288;
 
 struct ConvTcArgs {
   const float* bias;
@@ -73,33 +74,12 @@ __device__ __forceinline__ void tma_load_3d(uint32_t dst, const CUtensorMap* map
       : "memory");
 }
 
-// K-major, SWIZZLE_128B shared-memory matrix descriptor (cute::UMMA::SmemDescriptor layout):
-//   [0,14) start>>4 | [16,30) LBO>>4 (=1, unused for swizzled K-major) | [32,46) SBO>>4 (=64: 8 rows * 128 B)
-//   [46,48) version=1 (Blackwell) | [61,64) layout type 2 = SWIZZLE_128B
-__device__ __forceinline__ uint64_t make_sw128_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-
-__device__ __forceinline__ void umma_bf16(uint32_t tmem_d, uint64_t adesc, uint64_t bdesc, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(adesc), "l"(bdesc), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-
 template <int BN>
-__global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
-                                                             const __grid_constant__ CUtensorMap tmB, ConvTcArgs p) {
+__global__ void __launch_bounds__(TC_THREADS, 1) conv_tc_kernel(const __grid_constant__ CUtensorMap tmA,
+                                                                const __grid_constant__ CUtensorMap tmB, ConvTcArgs p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[TC_MAX_STAGES];
   __shared__ __align__(8) uint64_t bar_empty[TC_MAX_STAGES];
-  __shared__ __align__(8) uint64_t bar_acc;
-  __shared__ uint32_t tmem_slot;
 
   constexpr int B_BYTES = BN * TC_BK * 2;
   constexpr int STAGE_BYTES = TC_A_BYTES + B_BYTES;
@@ -120,28 +100,18 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mbar_init(smem_u32(&bar_full[s]), 1);
-      mbar_init(smem_u32(&bar_empty[s]), 1);
+      mbar_init(smem_u32(&bar_empty[s]), 8);  // one arrive per consumer warp
     }
-    mbar_init(smem_u32(&bar_acc), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
   }
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(&tmem_slot)), "n"(BN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       // ===== TMA producer =====
       for (int it = 0; it < total_k; ++it) {
@@ -157,84 +127,50 @@ __global__ void __launch_bounds__(TC_THREADS) conv_tc_kernel(const __grid_consta
         tma_load_3d(sa + TC_A_BYTES, &tmB, full, kb * TC_BK, n0, tap);
       }
     }
-  } else if (warp == 1) {
-    if (lane == 0) {
-      // ===== MMA issuer =====
-      // instruction descriptor (cute::UMMA::InstrDescriptor): c=F32 [4,6)=1, a=BF16 [7,10)=1, b=BF16 [10,13)=1,
-      // a/b K-major (bits 15,16 = 0), N>>3 at [17,23), M>>4 at [24,29)
-      constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(TC_BM >> 4) << 24);
-      for (int it = 0; it < total_k; ++it) {
-        const int s = it % S;
-        const uint32_t ph = (uint32_t)((it / S) & 1);
-        mbar_wait(smem_u32(&bar_full[s]), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sa = smem0 + (uint32_t)s * STAGE_BYTES;
-        const uint64_t adesc = make_sw128_desc(sa);
-        const uint64_t bdesc = make_sw128_desc(sa + TC_A_BYTES);
-#pragma unroll
-        for (int k = 0; k < TC_BK / 16; ++k) {
-          // advance 16 bf16 = 32 bytes along K inside the swizzle atom: +2 in the (addr>>4) field
-          umma_bf16(tmem_base, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), IDESC, (uint32_t)((it | k) != 0));
-        }
-        umma_commit(smem_u32(&bar_empty[s]));  // frees this smem stage when the MMAs above retire
-      }
-      umma_commit(smem_u32(&bar_acc));  // accumulator complete
-    }
   } else {
-    // ===== epilogue: TMEM -> registers -> (+bias, +residual) -> global fp32 NHWC =====
-    const int q = warp & 3;            // TMEM lane quadrant this warp may access
-    const int r = q * 32 + lane;       // accumulator row == pixel index inside the tile
-    const int ni = r / (p.th * p.tw);
-    const int rem = r - ni * (p.th * p.tw);
-    const int yy = rem / p.tw, xx = rem - yy * p.tw;
-    const int b = b0 + ni;
-    const bool valid = b < p.B;
-    const long long pix = ((long long)b * p.H + (y0 + yy)) * p.W + (x0 + xx);
-    float* __restrict__ orow = p.out + pix * p.Cout + n0;
-    const float* __restrict__ rrow = p.residual ? p.residual + pix * p.Cout + n0 : nullptr;
-    mbar_wait(smem_u32(&bar_acc), 0u);
-    asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-#pragma unroll 1
-    for (int c0 = 0; c0 < BN; c0 += 32) {
-      uint32_t v[32];
-      const uint32_t taddr = tmem_base + ((uint32_t)(q * 32) << 16) + (uint32_t)c0;
-      asm volatile(
-          "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-          "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-          : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-            "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-            "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-            "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-          : "r"(taddr)
-          : "memory");
-      asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-      if (valid) {
+    // ===== consumer warpgroup wg: rows [64 wg, 64 wg + 64) of the tile =====
+    const int wg = warp >> 2, t = threadIdx.x & 127;
+    float acc[BN / 2];
 #pragma unroll
-        for (int j = 0; j < 32; j += 4) {
-          float4 o;
-          o.x = __uint_as_float(v[j + 0]);
-          o.y = __uint_as_float(v[j + 1]);
-          o.z = __uint_as_float(v[j + 2]);
-          o.w = __uint_as_float(v[j + 3]);
-          if (p.bias) {
-            const float4 bv = __ldg(reinterpret_cast<const float4*>(p.bias + n0 + c0 + j));
-            o.x += bv.x; o.y += bv.y; o.z += bv.z; o.w += bv.w;
-          }
-          if (rrow) {
-            const float4 rv = *reinterpret_cast<const float4*>(rrow + c0 + j);
-            o.x += rv.x; o.y += rv.y; o.z += rv.z; o.w += rv.w;
-          }
-          *reinterpret_cast<float4*>(orow + c0 + j) = o;
-        }
-      }
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    int prev = -1;
+    for (int it = 0; it < total_k; ++it) {
+      const int s = it % S;
+      mbar_wait(smem_u32(&bar_full[s]), (uint32_t)((it / S) & 1));
+      const uint32_t sa = smem0 + (uint32_t)s * STAGE_BYTES;
+      const uint64_t adesc = wgmma::desc_sw128(sa + (uint32_t)wg * (64u * 128u), 16u, 1024u);
+      const uint64_t bdesc = wgmma::desc_sw128(sa + TC_A_BYTES, 16u, 1024u);
+      wgmma::fence();
+#pragma unroll
+      for (int k = 0; k < TC_BK / 16; ++k)  // 16 bf16 = 32 bytes along K inside the swizzle atom: +2 in the (addr>>4) field
+        wgmma::mma<BN, 0>(acc, adesc + (uint64_t)(2 * k), bdesc + (uint64_t)(2 * k), (uint32_t)((it | k) != 0));
+      wgmma::commit();
+      wgmma::wait<1>();  // the previous stage's MMAs have retired: release it
+      if (prev >= 0 && lane == 0) asm volatile("mbarrier.arrive.shared::cta.b64 _, [%0];" ::"r"(smem_u32(&bar_empty[prev])) : "memory");
+      prev = s;
     }
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 1) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(BN) : "memory");
+    wgmma::wait<0>();
+    // ===== epilogue: registers -> (+bias, +residual) -> global fp32 NHWC =====
+    const int ppi = p.th * p.tw;
+#pragma unroll
+    for (int i = 0; i < BN / 2; i += 2) {
+      const int r = 64 * wg + wgmma::frag_row(t, i), col = n0 + wgmma::frag_col(t, i);
+      const int ni = r / ppi, rem = r - ni * ppi;
+      const int yy = rem / p.tw, xx = rem - yy * p.tw;
+      const int b = b0 + ni;
+      if (b >= p.B) continue;
+      const long long pix = ((long long)b * p.H + (y0 + yy)) * p.W + (x0 + xx);
+      float2 o = make_float2(acc[i], acc[i + 1]);
+      if (p.bias) {
+        const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+        o.x += bv.x; o.y += bv.y;
+      }
+      if (p.residual) {
+        const float2 rv = *reinterpret_cast<const float2*>(p.residual + pix * p.Cout + col);
+        o.x += rv.x; o.y += rv.y;
+      }
+      *reinterpret_cast<float2*>(p.out + pix * p.Cout + col) = o;
+    }
   }
 }
 

@@ -1,20 +1,19 @@
-// conv_tc v2 -- persistent, warp-specialised tensor-core implicit-GEMM convolution for sm_100a.
+// conv_tc v2 -- persistent, warp-specialised tensor-core implicit-GEMM convolution for sm_90a.
 //
 //   warp 8   : TMA producer  (4-D activation boxes with OOB zero fill = conv padding, 3-D weight boxes)
-//   warp 9   : tcgen05.mma issuer; accumulators are DOUBLE-BUFFERED in TMEM (2 x BN columns), so
-//   warps 0-7: (two groups) the epilogue of tile i overlaps the main loop of tile i+1:
-//   (the two single-thread roles have the HIGHEST warp ids: the scheduler favours higher ids among eligible warps, so the
-//    issuer / producer are not starved of issue slots by the eight epilogue warps)
-//              tcgen05.ld -> +bias (+fp32 residual fetched by TMA) -> 128B-swizzled staging tile in smem ->
+//   warps 0-7: two consumer warpgroups; warpgroup g owns rows [64 g, 64 g + 64) of every 128-pixel tile:
+//              wgmma (bf16 x bf16 -> fp32 accumulators in registers) over the stage ring, then the epilogue straight
+//              from the accumulator fragments: +bias (+residual fetched by TMA) -> 128B-swizzled staging tile in smem ->
 //              per-channel GroupNorm partial sums (sum, sum^2) -> TMA store (fp32 or bf16 NHWC).
-// One CTA per SM, static round-robin tile schedule (tile = blockIdx.x + i * gridDim.x; all CTAs sweep the same
-// weight tile at the same time, so it stays hot in L2).
+// One CTA per SM, contiguous tile range per CTA (consecutive tiles mostly share an image and the weight tile).  The producer
+// runs ahead into the next tile while the consumers are in the epilogue.
 //
 // The BN=16 instantiation is the UNet image head (Cout=3 zero-padded to 16): it skips the TMA store and writes the
-// first `cout_valid` columns as NCHW fp32 planes (coalesced along x).
+// first `cout_valid` columns as NCHW fp32 planes.
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pdae {
 
@@ -23,8 +22,8 @@ constexpr int T2_BK = 64;
 constexpr int T2_A_BYTES = T2_BM * T2_BK * 2;  // 16 KB
 constexpr int T2_STG_BYTES = 128 * 128;        // staging tile: 128 rows x 128 B
 constexpr int T2_MAX_STAGES = 8;
-constexpr int T2_THREADS = 320;   // warp 0 TMA, warp 1 MMA, warps 2-5 / 6-9 = two epilogue groups (one per TMEM accumulator)
-constexpr int T2_EPI_THREADS = 128;
+constexpr int T2_THREADS = 288;   // warps 0-7: two consumer warpgroups, warp 8: TMA producer
+constexpr int T2_CONSUMERS = 256;
 
 struct ConvTc2Args {
   const float* bias;
@@ -43,9 +42,7 @@ struct ConvTc2Args {
   int w_stat;     // weights stationary: every B tile of the (single) n-tile is loaded ONCE per CTA into its own shared-memory
                   // region and reused by all of the CTA's tiles; pipeline stages then hold A tiles only
   float softmax_alpha;  // > 0: the epilogue stores softmax_row(alpha * acc) (bf16) instead of acc -- attention scores whose
-                        // whole row lives in this tile's TMEM accumulator (N == BN); model/module.py:452-455,483-486
-  int dbg_shift;  // probe (scripts/desc_shift_probe.py): load the A box dbg_shift pixels EARLY and start the UMMA descriptor
-  int dbg_boff;   // dbg_shift rows (x 128 B) into it, with the descriptor's base_offset field = dbg_boff -- 0 in production
+                        // whole row lives in this tile's accumulators (N == BN); model/module.py:452-455,483-486
 };
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -70,9 +67,8 @@ __device__ __forceinline__ uint32_t mb_try(uint32_t bar, uint32_t parity) {
   return done;
 }
 // Slow path of a wait: mbarrier.try_wait with a SUSPEND-TIME HINT, so a waiting warp sleeps in hardware (it is woken by the
-// completing arrive) instead of re-issuing the poll every ~100 cycles.  With 18+ warps per CTA of which most are waiting at
-// any time, hot polling took more than half of all issue slots away from the warps that had work (ncu: 8.4 M polls per
-// launch, profiles/r02_ncu_conv_tc3_spin.txt).
+// completing arrive) instead of re-issuing the poll: most of the CTA's warps are waiting at any time, and hot polling takes
+// issue slots away from the warps that have work.
 __device__ __forceinline__ uint32_t mb_try_sleep(uint32_t bar, uint32_t parity) {
   uint32_t done;
   asm volatile(
@@ -110,54 +106,21 @@ __device__ __forceinline__ void tma_st4(const CUtensorMap* m, uint32_t src, int 
                "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
-__device__ __forceinline__ uint64_t sw128_desc(uint32_t saddr) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | (64ull << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(a), "l"(b), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_to(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 // One elected lane of a fully converged warp: the producer / issuer loops run on all 32 lanes (warp-uniform operands stay in
-// uniform registers); only the TMA / tcgen05 instruction is predicated.  Under `if (lane == 0)` every descriptor was a
+// uniform registers); only the TMA instruction is predicated.  Under `if (lane == 0)` every descriptor was a
 // per-lane value and each MMA paid an ELECT + 5 x R2UR.BROADCAST + branch waterfall.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void epi_bar(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
-
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
-__device__ __forceinline__ void tmem_ld16(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x16.b32 {%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15}, [%16];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15])
-      : "r"(taddr)
-      : "memory");
-}
+// barrier of the 256 consumer threads (the producer warp never joins it)
+__device__ __forceinline__ void cons_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 
 // byte offset of (row, 16-byte chunk) inside a 128-row x 128-byte SWIZZLE_128B staging tile
 __device__ __forceinline__ uint32_t swz(int row, int chunk16) { return (uint32_t)(row * 128 + ((chunk16 ^ (row & 7)) << 4)); }
 
-template <int BN>
+template <int BN, bool OB>
 __global__ void __launch_bounds__(T2_THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
@@ -165,19 +128,21 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                 const __grid_constant__ CUtensorMap tmA3, ConvTc2Args p) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[T2_MAX_STAGES], bar_empty[T2_MAX_STAGES];
-  __shared__ __align__(8) uint64_t bar_acc_full[2], bar_acc_empty[2], bar_res[2], bar_w;
-  __shared__ uint32_t tmem_slot;
-  __shared__ float st_acc[2][2][BN < 32 ? 32 : BN];  // [epilogue group][sum | sum^2][channel] of the group's current (image, n-tile)
+  __shared__ __align__(8) uint64_t bar_res, bar_w;
+  __shared__ float st_acc[2][BN < 32 ? 32 : BN];  // [sum | sum^2][channel] of the current (image, n-tile)
+  __shared__ float st_part[2][8][32];              // per-chunk partial sums [sum | sum^2][row run][column] (CW * 8 runs / 32)
 
   constexpr int B_BYTES = BN * T2_BK * 2;
   constexpr int STAGE_BYTES = T2_A_BYTES + ((B_BYTES + 1023) / 1024) * 1024;
-  constexpr int TMEM_COLS = (2 * BN < 32) ? 32 : 2 * BN;
+  constexpr int CW = OB ? 64 : 32;             // accumulator columns per staging tile (128-byte rows)
+  constexpr int NCH = BN < CW ? 1 : BN / CW;
+  constexpr int RPT = CW / 2;                  // statistics: rows per thread (256 threads = CW columns x 128 / RPT row runs)
   const uint32_t smem0 = (s_u32(smem_raw) + 1023u) & ~1023u;
   const int S = p.stages;
   const uint32_t stage_stride = p.w_stat ? (uint32_t)T2_A_BYTES : (uint32_t)STAGE_BYTES;
   const uint32_t wbase = smem0 + (uint32_t)S * stage_stride;                       // stationary weights (w_stat only)
-  const uint32_t stg_out = wbase + (p.w_stat ? (uint32_t)((p.taps * p.kblocks + p.kblocks2) * B_BYTES) : 0u);   // 2 x 16 KB output staging   (one per epilogue group)
-  const uint32_t stg_res = stg_out + 2u * T2_STG_BYTES;         // 2 x 16 KB residual staging (one per group; only if has_res)
+  const uint32_t stg_out = wbase + (p.w_stat ? (uint32_t)((p.taps * p.kblocks + p.kblocks2) * B_BYTES) : 0u);   // 16 KB output staging
+  const uint32_t stg_res = stg_out + (uint32_t)T2_STG_BYTES;   // 16 KB residual staging (only if has_res)
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_k = p.taps * p.kblocks;          // main conv
   const int total_all = total_k + p.kblocks2;      // + fused 1x1 skip conv
@@ -188,35 +153,22 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int tile_end = min(p.tiles_total, tile_begin + per_cta);
 
   for (int j = threadIdx.x; j < (BN < 32 ? 32 : BN); j += T2_THREADS) {
-    st_acc[0][0][j] = 0.f; st_acc[0][1][j] = 0.f;
-    st_acc[1][0][j] = 0.f; st_acc[1][1][j] = 0.f;
+    st_acc[0][j] = 0.f;
+    st_acc[1][j] = 0.f;
   }
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mb_init(s_u32(&bar_full[s]), 1);
-      mb_init(s_u32(&bar_empty[s]), 1);
+      mb_init(s_u32(&bar_empty[s]), 8);   // one arrive per consumer warp
     }
-    for (int i = 0; i < 2; ++i) {
-      mb_init(s_u32(&bar_acc_full[i]), 1);
-      mb_init(s_u32(&bar_acc_empty[i]), 1);
-      mb_init(s_u32(&bar_res[i]), 1);
-    }
+    mb_init(s_u32(&bar_res), 1);
     mb_init(s_u32(&bar_w), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
-  if (warp == 9) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(&tmem_slot)), "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_slot;
 
   if (warp == 8) {
     // ================= TMA producer (warp-uniform loop, elected lane issues) =================
@@ -250,7 +202,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
         if (elect_one()) {
           mb_expect_tx(full, stage_tx);
-          tma_ld4(sa, &tmA, full, kb * T2_BK, x0 + dx - p.dbg_shift, y0 + dy, b0);
+          tma_ld4(sa, &tmA, full, kb * T2_BK, x0 + dx, y0 + dy, b0);
           if (!ws) tma_ld3(sa + T2_A_BYTES, &tmB, full, kb * T2_BK, n0, p.w_batched ? b0 : tap);
         }
         __syncwarp();
@@ -275,53 +227,23 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         if (++s == S) { s = 0; ph ^= 1u; }
       }
     }
-  } else if (warp == 9) {
-    // ================= MMA issuer (warp-uniform loop, elected lane issues) =================
-    constexpr uint32_t IDESC =
-        (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(T2_BM >> 4) << 24);
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    int s = 0, tl = 0;
-    uint32_t ph = 0;
-    if (p.w_stat && tile_begin < tile_end) mb_wait(s_u32(&bar_w), 0u);   // stationary weights have landed
-    for (int tile = tile_begin; tile < tile_end; ++tile, ++tl) {
-      const int ab = tl & 1;
-      mb_wait(s_u32(&bar_acc_empty[ab]), (uint32_t)(((tl >> 1) & 1) ^ 1));  // epilogue drained this accumulator
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tmem_d = tmem_u + (uint32_t)(ab * BN);
-      for (int it = 0; it < total_all; ++it) {
-        mb_wait(s_u32(&bar_full[s]), ph);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
-        const uint64_t ad = sw128_desc(sa + (uint32_t)p.dbg_shift * 128u) | ((uint64_t)p.dbg_boff << 49),
-                       bd = sw128_desc(p.w_stat ? wbase + (uint32_t)(it * B_BYTES) : sa + T2_A_BYTES);
-        const uint32_t first = (uint32_t)(it != 0);
-        const uint32_t bar_e = s_u32(&bar_empty[s]);
-        if (elect_one()) {
-          umma(tmem_d, ad, bd, IDESC, first);
-#pragma unroll
-          for (int k = 1; k < T2_BK / 16; ++k) umma(tmem_d, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), IDESC, 1u);
-          umma_commit_to(bar_e);
-        }
-        __syncwarp();
-        if (++s == S) { s = 0; ph ^= 1u; }
-      }
-      if (elect_one()) umma_commit_to(s_u32(&bar_acc_full[ab]));
-      __syncwarp();
-    }
   } else {
-    // ================= epilogue: two groups of 128 threads; group g drains accumulator buffer g =================
-    // (tile tl of this CTA lands in accumulator tl & 1, so the groups work on alternate tiles concurrently: the per-tile
-    //  epilogue chain -- tcgen05.ld, residual, staging, TMA store, statistics -- has twice the throughput)
-    const int eg = warp >> 2;                  // epilogue group 0 | 1
-    const int et = threadIdx.x - eg * 128;     // 0..127 inside the group
-    const bool elected = et == 0;
-    const int q = warp & 3;                    // TMEM lane quadrant of this warp
-    const int r = q * 32 + lane;               // accumulator row = pixel index in the tile
+    // ================= consumers: warpgroup wg computes rows [64 wg, 64 wg + 64) of each tile, then both run the epilogue ==========
+    const int wg = warp >> 2;
+    const int t = threadIdx.x & 127;           // thread inside the warpgroup (accumulator fragment owner)
+    const int ct = threadIdx.x;                // 0..255 over both warpgroups
+    const bool elected = ct == 0;
     const int ppi = p.th * p.tw;               // pixels per image inside a tile
-    int rc = 0;                                // residual loads consumed by this group (mbarrier phase)
-    const uint32_t obuf = stg_out + (uint32_t)eg * T2_STG_BYTES, rbuf = stg_res + (uint32_t)eg * T2_STG_BYTES;
-    const uint32_t rbar = s_u32(&bar_res[eg]);
-    for (int tile = tile_begin + eg, tl = eg; tile < tile_end; tile += 2, tl += 2) {
+    int rc = 0;                                // residual loads consumed (mbarrier phase)
+    int s = 0;
+    uint32_t ph = 0;
+    const uint32_t obuf = stg_out, rbuf = stg_res;
+    const uint32_t rbar = s_u32(&bar_res);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    if (p.w_stat && tile_begin < tile_end) mb_wait(s_u32(&bar_w), 0u);   // stationary weights have landed
+    for (int tile = tile_begin; tile < tile_end; ++tile) {
       const int nt = tile / p.tiles_m;
       int mt = tile - nt * p.tiles_m;
       const int tx = mt % p.tiles_x;
@@ -329,36 +251,52 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       const int ty = mt % p.tiles_y;
       const int bt = mt / p.tiles_y;
       const int x0 = tx * p.tw, y0 = ty * p.th, b0 = bt * p.tn, n0 = nt * BN;
-      const int ab = tl & 1;
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(ab * BN) + ((uint32_t)(q * 32) << 16);
-      mb_wait(s_u32(&bar_acc_full[ab]), (uint32_t)((tl >> 1) & 1));
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
+      if constexpr (BN != 16) {
+        if (p.has_res && elected) {            // residual chunk 0 of this tile (lands while the main loop runs)
+          mb_expect_tx(rbar, T2_STG_BYTES);
+          tma_ld4(rbuf, &tmR, rbar, n0, x0, y0, b0);
+        }
+      }
+      // ---- main loop: wgmma over the stage ring; a stage is released once the MMAs reading it have retired ----
+      int prev = -1;
+      for (int it = 0; it < total_all; ++it) {
+        mb_wait(s_u32(&bar_full[s]), ph);
+        const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
+        const uint64_t ad = wgmma::desc_sw128(sa + (uint32_t)wg * (64u * 128u), 16u, 1024u);
+        const uint64_t bd = wgmma::desc_sw128(p.w_stat ? wbase + (uint32_t)(it * B_BYTES) : sa + T2_A_BYTES, 16u, 1024u);
+        wgmma::fence();
+#pragma unroll
+        for (int k = 0; k < T2_BK / 16; ++k)
+          wgmma::mma<BN, 0>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (uint32_t)((it | k) != 0));
+        wgmma::commit();
+        wgmma::wait<1>();
+        if (prev >= 0 && lane == 0) mb_arrive(s_u32(&bar_empty[prev]));
+        prev = s;
+        if (++s == S) { s = 0; ph ^= 1u; }
+      }
+      wgmma::wait<0>();
+      if (prev >= 0 && lane == 0) mb_arrive(s_u32(&bar_empty[prev]));
 
       if constexpr (BN == 16) {
         // ---- image head: first cout_valid columns -> NCHW fp32 planes ----
-        uint32_t v[16];
-        tmem_ld16(tmem_acc, v);
-        asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-        const int ni = r / ppi, rem = r - ni * ppi;
-        const int yy = rem / p.tw, xx = rem - yy * p.tw;
-        const int b = b0 + ni;
-        if (b < p.B) {
-          const long long hw = (long long)p.H * p.W;
-          const long long pix = (long long)(y0 + yy) * p.W + (x0 + xx);
-          float* o = p.out_nchw + (long long)b * p.cout_valid * hw + pix;
-          float val[16];
+        const long long hw = (long long)p.H * p.W;
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            val[j] = __uint_as_float(v[j]) + (p.bias ? __ldg(p.bias + j) : 0.f);
-            if (j < p.cout_valid) o[j * hw] = val[j];
-          }
+        for (int i = 0; i < BN / 2; ++i) {
+          const int r = 64 * wg + wgmma::frag_row(t, i), j = wgmma::frag_col(t, i);
+          const int ni = r / ppi, rem = r - ni * ppi;
+          const int yy = rem / p.tw, xx = rem - yy * p.tw;
+          const int b = b0 + ni;
+          if (b >= p.B) continue;
+          const long long pix = (long long)(y0 + yy) * p.W + (x0 + xx);
+          const float val = acc[i] + (p.bias ? __ldg(p.bias + j) : 0.f);
+          if (j < p.cout_valid) p.out_nchw[((long long)b * p.cout_valid + j) * hw + pix] = val;
           // ---- fused DDIM update (diffusion/ddim.py:43-55, 66-79, 91-107, 123-138): this head's output is the last tensor the
           // step needs, so x_t -> x_{t-1} (or x_{t+1}) is finished here, in place, with the exact arithmetic of ddim_step_kernel.
           // The descriptor lives in device memory and is (re)written by the sampling loop; flags == 0 -> plain head conv.
           if (p.fuse) {
             const long long flags = __ldg(p.fuse);
-            if (flags & 1) {
-              const int C = (int)((flags >> 8) & 0xff), Ce = (int)((flags >> 16) & 0xff);
+            const int C = (int)((flags >> 8) & 0xff), Ce = (int)((flags >> 16) & 0xff);
+            if ((flags & 1) && j < C) {
               const float* eps = reinterpret_cast<const float*>(__ldg(p.fuse + 1));
               float* xt = reinterpret_cast<float*>(__ldg(p.fuse + 2));
               const long long tb = reinterpret_cast<const long long*>(__ldg(p.fuse + 3))[b];
@@ -366,149 +304,109 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               const float Bm = reinterpret_cast<const float*>(__ldg(p.fuse + 5))[tb];
               const float abar = reinterpret_cast<const float*>(__ldg(p.fuse + 7))[tb];
               const float s1m = (flags & 2) ? reinterpret_cast<const float*>(__ldg(p.fuse + 6))[tb] : 0.f;
-#pragma unroll
-              for (int j = 0; j < 16; ++j) {
-                if (j < C) {
-                  const long long xi = ((long long)b * C + j) * hw + pix;
-                  float e = val[j];                                  // this head predicts epsilon itself
-                  if (flags & 2) e = __fsub_rn(eps[((long long)b * Ce + j) * hw + pix], __fmul_rn(s1m, val[j]));   // own output = shift term
-                  else if (flags & 4) e = eps[((long long)b * Ce + j) * hw + pix];   // shift unused this step: epsilon from the other head
-                  const float ax = __fmul_rn(A, xt[xi]);
-                  float x0 = __fsub_rn(ax, __fmul_rn(Bm, e));
-                  x0 = fminf(fmaxf(x0, -1.0f), 1.0f);
-                  const float e2 = __fdiv_rn(__fsub_rn(ax, x0), Bm);
-                  xt[xi] = __fadd_rn(__fmul_rn(x0, sqrtf(abar)), __fmul_rn(sqrtf(__fsub_rn(1.0f, abar)), e2));
-                }
-              }
+              const long long xi = ((long long)b * C + j) * hw + pix;
+              float e = val;                                  // this head predicts epsilon itself
+              if (flags & 2) e = __fsub_rn(eps[((long long)b * Ce + j) * hw + pix], __fmul_rn(s1m, val));   // own output = shift term
+              else if (flags & 4) e = eps[((long long)b * Ce + j) * hw + pix];   // shift unused this step: epsilon from the other head
+              const float ax = __fmul_rn(A, xt[xi]);
+              float x0v = __fsub_rn(ax, __fmul_rn(Bm, e));
+              x0v = fminf(fmaxf(x0v, -1.0f), 1.0f);
+              const float e2 = __fdiv_rn(__fsub_rn(ax, x0v), Bm);
+              xt[xi] = __fadd_rn(__fmul_rn(x0v, sqrtf(abar)), __fmul_rn(sqrtf(__fsub_rn(1.0f, abar)), e2));
             }
           }
         }
       } else {
-        const int CW = p.out_bf16 ? 64 : 32;  // accumulator columns per staging tile (128-byte rows)
-        const int nch = BN / CW;
-        if (p.has_res && elected) {            // residual chunk 0 of this tile (issued before the accumulator is needed)
-          mb_expect_tx(rbar, T2_STG_BYTES);
-          tma_ld4(rbuf, &tmR, rbar, n0, x0, y0, b0);
-        }
-        // softmax epilogue: three passes over the accumulator row held in TMEM (max, sum of exp, normalised store)
-        float sm_mx = 0.f, sm_inv = 1.f;
-        const float sm_a = p.softmax_alpha * 1.4426950408889634f;
         if (p.softmax_alpha > 0.f) {
-          float mx = -3.0e38f;
-          for (int c2 = 0; c2 < BN / 32; ++c2) {
-            uint32_t v[32];
-            tmem_ld32(tmem_acc + (uint32_t)(c2 * 32), v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+          // softmax epilogue: the thread's two rows (i / 2 % 2) are spread over the 4 lanes of a quad
+          const float sm_a = p.softmax_alpha * 1.4426950408889634f;
+          float mx[2] = {-3.0e38f, -3.0e38f}, sum[2] = {0.f, 0.f};
 #pragma unroll
-            for (int j = 0; j < 32; ++j) mx = fmaxf(mx, __uint_as_float(v[j]));
-          }
-          float sum = 0.f;
-          for (int c2 = 0; c2 < BN / 32; ++c2) {
-            uint32_t v[32];
-            tmem_ld32(tmem_acc + (uint32_t)(c2 * 32), v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+          for (int i = 0; i < BN / 2; ++i) mx[(i >> 1) & 1] = fmaxf(mx[(i >> 1) & 1], acc[i]);
 #pragma unroll
-            for (int j = 0; j < 32; ++j) sum += exp2f((__uint_as_float(v[j]) - mx) * sm_a);
+          for (int h = 0; h < 2; ++h) {
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 1));
+            mx[h] = fmaxf(mx[h], __shfl_xor_sync(0xffffffffu, mx[h], 2));
           }
-          sm_mx = mx;
-          sm_inv = 1.0f / sum;
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) sum[(i >> 1) & 1] += exp2f((acc[i] - mx[(i >> 1) & 1]) * sm_a);
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 1);
+            sum[h] += __shfl_xor_sync(0xffffffffu, sum[h], 2);
+            sum[h] = 1.0f / sum[h];
+          }
+#pragma unroll
+          for (int i = 0; i < BN / 2; ++i) acc[i] = exp2f((acc[i] - mx[(i >> 1) & 1]) * sm_a) * sum[(i >> 1) & 1];
         }
-        for (int c = 0; c < nch; ++c) {
-          float val[64];
-          {
-            uint32_t v[32];
-            tmem_ld32(tmem_acc + (uint32_t)(c * CW), v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
 #pragma unroll
-            for (int j = 0; j < 32; ++j) val[j] = __uint_as_float(v[j]);
-            if (p.out_bf16) {
-              tmem_ld32(tmem_acc + (uint32_t)(c * CW + 32), v);
-              asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+        for (int c = 0; c < NCH; ++c) {
+          // this chunk's fragment registers: i in [c CW/2, (c+1) CW/2), column inside the chunk = frag_col - c CW
+          float v[CW / 2];
 #pragma unroll
-              for (int j = 0; j < 32; ++j) val[32 + j] = __uint_as_float(v[j]);
-            }
-          }
-          if (p.softmax_alpha > 0.f) {
-#pragma unroll
-            for (int j = 0; j < 64; ++j) val[j] = exp2f((val[j] - sm_mx) * sm_a) * sm_inv;
-          }
+          for (int q = 0; q < CW / 2; ++q) v[q] = acc[c * (CW / 2) + q];
           if (p.bias) {
-            const float4* bp = reinterpret_cast<const float4*>(p.bias + n0 + c * CW);
 #pragma unroll
-            for (int j = 0; j < 16; ++j) {
-              if (j * 4 < CW) {
-                const float4 bv = __ldg(bp + j);
-                val[4 * j + 0] += bv.x; val[4 * j + 1] += bv.y; val[4 * j + 2] += bv.z; val[4 * j + 3] += bv.w;
-              }
+            for (int q = 0; q < CW / 2; q += 2) {
+              const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c * CW + wgmma::frag_col(t, q)));
+              v[q] += bv.x; v[q + 1] += bv.y;
             }
           }
           if (p.has_res) {                      // the residual has the output's dtype: CW columns = one 128-byte row
             mb_wait(rbar, (uint32_t)(rc & 1));
-            if (p.out_bf16) {
 #pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                uint32_t w[4];
-                asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3])
-                             : "r"(rbuf + swz(r, j)));
-#pragma unroll
-                for (int h = 0; h < 4; ++h) {
-                  val[8 * j + 2 * h] += __uint_as_float(w[h] << 16);
-                  val[8 * j + 2 * h + 1] += __uint_as_float(w[h] & 0xffff0000u);
-                }
-              }
-            } else {
-#pragma unroll
-              for (int j = 0; j < 8; ++j) {
-                float4 rv;
-                asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(rv.x), "=f"(rv.y), "=f"(rv.z), "=f"(rv.w)
-                             : "r"(rbuf + swz(r, j)));
-                val[4 * j + 0] += rv.x; val[4 * j + 1] += rv.y; val[4 * j + 2] += rv.z; val[4 * j + 3] += rv.w;
+            for (int q = 0; q < CW / 2; q += 2) {
+              const int r = 64 * wg + wgmma::frag_row(t, q), cl = wgmma::frag_col(t, q);
+              if (OB) {
+                uint32_t w;
+                asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(rbuf + swz(r, cl >> 3) + (uint32_t)((cl & 7) * 2)));
+                v[q] += __uint_as_float(w << 16);
+                v[q + 1] += __uint_as_float(w & 0xffff0000u);
+              } else {
+                float2 rv;
+                asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(rv.x), "=f"(rv.y)
+                             : "r"(rbuf + swz(r, cl >> 2) + (uint32_t)((cl & 3) * 4)));
+                v[q] += rv.x; v[q + 1] += rv.y;
               }
             }
             ++rc;
           }
-          // the group's staging buffer must no longer be read by its previous TMA store
+          // the staging buffer must no longer be read by the previous TMA store
           if (elected) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");
-          epi_bar(eg);                          // (also: every thread has consumed the residual buffer)
-          if (p.has_res && elected && c + 1 < nch) {   // residual for the next chunk overlaps this chunk's store + statistics
+          cons_bar();                           // (also: every thread has consumed the residual buffer)
+          if (p.has_res && elected && c + 1 < NCH) {   // residual for the next chunk overlaps this chunk's store + statistics
             mb_expect_tx(rbar, T2_STG_BYTES);
             tma_ld4(rbuf, &tmR, rbar, n0 + (c + 1) * CW, x0, y0, b0);
           }
-          if (p.out_bf16) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              uint32_t w[4];
-#pragma unroll
-              for (int h = 0; h < 4; ++h) {
-                __nv_bfloat162 b2 = __floats2bfloat162_rn(val[8 * j + 2 * h], val[8 * j + 2 * h + 1]);
-                w[h] = *reinterpret_cast<uint32_t*>(&b2);
-              }
-              asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(obuf + swz(r, j)), "r"(w[0]), "r"(w[1]), "r"(w[2]),
-                           "r"(w[3])
+          for (int q = 0; q < CW / 2; q += 2) {
+            const int r = 64 * wg + wgmma::frag_row(t, q), cl = wgmma::frag_col(t, q);
+            if (OB) {
+              __nv_bfloat162 b2 = __floats2bfloat162_rn(v[q], v[q + 1]);
+              asm volatile("st.shared.b32 [%0], %1;" ::"r"(obuf + swz(r, cl >> 3) + (uint32_t)((cl & 7) * 2)),
+                           "r"(*reinterpret_cast<uint32_t*>(&b2))
+                           : "memory");
+            } else {
+              asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(obuf + swz(r, cl >> 2) + (uint32_t)((cl & 3) * 4)), "f"(v[q]),
+                           "f"(v[q + 1])
                            : "memory");
             }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j)
-              asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(obuf + swz(r, j)), "f"(val[4 * j]), "f"(val[4 * j + 1]),
-                           "f"(val[4 * j + 2]), "f"(val[4 * j + 3])
-                           : "memory");
           }
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-          epi_bar(eg);
+          cons_bar();
           if (elected) {
             tma_st4(&tmO, obuf, n0 + c * CW, x0, y0, b0);
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
           }
           if (p.ch_stats) {
             // per-channel partial sums over this tile's rows, read back from the staged (rounded) values:
-            // thread -> column (et % CW), rows [(et / CW) * CW, +CW)
-            const int col = et % CW, r0 = (et / CW) * CW;
-            const uint32_t cbyte = p.out_bf16 ? (uint32_t)((col & 7) * 2) : (uint32_t)((col & 3) * 4);
-            const int cchunk = p.out_bf16 ? (col >> 3) : (col >> 2);
+            // thread -> column (ct % CW), rows [(ct / CW) * RPT, +RPT)
+            const int col = ct % CW, r0 = (ct / CW) * RPT;
+            const uint32_t cbyte = OB ? (uint32_t)((col & 7) * 2) : (uint32_t)((col & 3) * 4);
+            const int cchunk = OB ? (col >> 3) : (col >> 2);
             auto ldv = [&](int rr) -> float {
               float x;
-              if (p.out_bf16) {
+              if (OB) {
                 unsigned short h;
                 asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(obuf + swz(rr, cchunk) + cbyte));
                 x = __uint_as_float(((uint32_t)h) << 16);
@@ -518,95 +416,96 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               return x;
             };
             if (p.tn == 1) {
-              // whole tile = one image: accumulate in shared memory across this CTA's consecutive tiles
-              float s = 0.f, qq = 0.f;
+              // whole tile = one image: accumulate in shared memory across this CTA's consecutive tiles.  The row runs of a
+              // column are added in a fixed order by one thread, so repeated runs give identical statistics.
+              float sacc = 0.f, qq = 0.f;
 #pragma unroll 8
-              for (int rr = r0; rr < r0 + CW; ++rr) {
+              for (int rr = r0; rr < r0 + RPT; ++rr) {
                 const float x = ldv(rr);
-                s += x;
+                sacc += x;
                 qq = fmaf(x, x, qq);
               }
-              atomicAdd(&st_acc[eg][0][c * CW + col], s);
-              atomicAdd(&st_acc[eg][1][c * CW + col], qq);
-            } else if (ppi % CW == 0) {
-              // several whole images per tile and this thread's CW rows lie inside ONE image
-              float s = 0.f, qq = 0.f;
+              float* part = &st_part[0][0][0];
+              part[ct] = sacc;
+              part[256 + ct] = qq;
+              cons_bar();
+              if (ct < CW) {
+                float s2 = 0.f, q2 = 0.f;
+#pragma unroll
+                for (int g = 0; g < 256 / CW; ++g) {
+                  s2 += part[g * CW + ct];
+                  q2 += part[256 + g * CW + ct];
+                }
+                st_acc[0][c * CW + ct] += s2;
+                st_acc[1][c * CW + ct] += q2;
+              }
+            } else if (ppi % RPT == 0) {
+              // several whole images per tile and this thread's RPT rows lie inside ONE image
+              float sacc = 0.f, qq = 0.f;
 #pragma unroll 8
-              for (int rr = r0; rr < r0 + CW; ++rr) {
+              for (int rr = r0; rr < r0 + RPT; ++rr) {
                 const float x = ldv(rr);
-                s += x;
+                sacc += x;
                 qq = fmaf(x, x, qq);
               }
               const int cur = r0 / ppi;
               if (b0 + cur < p.B) {
                 float* dst = p.ch_stats + ((long long)(b0 + cur) * p.Cout + n0 + c * CW + col) * 2;
-                if (ppi == CW && p.tiles_x * p.tiles_y == 1) {   // whole image inside this tile and this thread covers all of
+                if (ppi == RPT && p.tiles_x * p.tiles_y == 1) {  // whole image inside this tile and this thread covers all of
                                                                  // its rows: the only contributor -> plain store, no atomic
-                  *reinterpret_cast<float2*>(dst) = make_float2(s, qq);
+                  *reinterpret_cast<float2*>(dst) = make_float2(sacc, qq);
                 } else {
-                  atomicAdd(dst, s);
+                  atomicAdd(dst, sacc);
                   atomicAdd(dst + 1, qq);
                 }
               }
             } else {
-              float s = 0.f, qq = 0.f;
+              float sacc = 0.f, qq = 0.f;
               int cur = r0 / ppi, nxt = (cur + 1) * ppi;  // `nxt` = first row of the next image
               float* dst0 = p.ch_stats + ((long long)b0 * p.Cout + n0 + c * CW + col) * 2;
-              for (int rr = r0; rr < r0 + CW; ++rr) {
+              for (int rr = r0; rr < r0 + RPT; ++rr) {
                 if (rr == nxt) {
                   if (b0 + cur < p.B) {
-                    atomicAdd(dst0 + (long long)cur * p.Cout * 2, s);
+                    atomicAdd(dst0 + (long long)cur * p.Cout * 2, sacc);
                     atomicAdd(dst0 + (long long)cur * p.Cout * 2 + 1, qq);
                   }
-                  s = qq = 0.f;
+                  sacc = qq = 0.f;
                   ++cur;
                   nxt += ppi;
                 }
                 const float x = ldv(rr);
-                s += x;
+                sacc += x;
                 qq = fmaf(x, x, qq);
               }
               if (b0 + cur < p.B) {
-                atomicAdd(dst0 + (long long)cur * p.Cout * 2, s);
+                atomicAdd(dst0 + (long long)cur * p.Cout * 2, sacc);
                 atomicAdd(dst0 + (long long)cur * p.Cout * 2 + 1, qq);
               }
             }
           }
         }
-      }
-      // accumulator buffer fully read by every epilogue thread -> hand it back to the MMA warp
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      epi_bar(eg);
-      if (elected) mb_arrive(s_u32(&bar_acc_empty[ab]));
-      if constexpr (BN != 16) {
         if (p.ch_stats && p.tn == 1) {
-          bool flush = tile + 2 >= tile_end;     // this group's next tile is tile + 2
+          bool flush = tile + 1 >= tile_end;
           if (!flush) {
-            const int nt2 = (tile + 2) / p.tiles_m;
-            const int bt2 = ((tile + 2) - nt2 * p.tiles_m) / (p.tiles_x * p.tiles_y);
+            const int nt2 = (tile + 1) / p.tiles_m;
+            const int bt2 = ((tile + 1) - nt2 * p.tiles_m) / (p.tiles_x * p.tiles_y);
             flush = nt2 != nt || bt2 != bt;
           }
-          if (flush) {  // (the epi_bar above ordered every thread's shared-memory atomics before these reads)
-            for (int j = et; j < BN; j += 128) {
+          if (flush) {
+            cons_bar();   // every thread's shared-memory atomics are done before these reads
+            for (int j = ct; j < BN; j += T2_CONSUMERS) {
               float* dst = p.ch_stats + ((long long)b0 * p.Cout + n0 + j) * 2;
-              atomicAdd(dst, st_acc[eg][0][j]);
-              atomicAdd(dst + 1, st_acc[eg][1][j]);
-              st_acc[eg][0][j] = 0.f;
-              st_acc[eg][1][j] = 0.f;
+              atomicAdd(dst, st_acc[0][j]);
+              atomicAdd(dst + 1, st_acc[1][j]);
+              st_acc[0][j] = 0.f;
+              st_acc[1][j] = 0.f;
             }
-            epi_bar(eg);
+            cons_bar();
           }
         }
       }
     }
     if (elected) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 9) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
   }
 }
 
@@ -633,17 +532,17 @@ static int pow2_tile(int W, int cap) {
   return t;
 }
 
-template <int BN>
+template <int BN, bool OB>
 static cudaError_t launch_tc2(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r,
                               const CUtensorMap& a2, const CUtensorMap& b2, const CUtensorMap& a3, const ConvTc2Args& args,
                               int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, 2 x per-group stats <= 4 KB) <= 227 KB
+    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, OB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, stats <= 2 KB) <= 227 KB
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  conv_tc2_kernel<BN><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args);
+  conv_tc2_kernel<BN, OB><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args);
   return cudaPeekAtLastError();
 }
 
@@ -721,16 +620,11 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
     delete pl;
     PDAE_REQUIRE(false, "conv_tc2_create: the softmax epilogue needs a bf16 batched GEMM whose row fits one tile (N=%d)", Cout);
   }
-  {   // descriptor row-shift probe knobs (never set in production)
-    const char* e1 = getenv("PDAE_TC_DBG_SHIFT");
-    const char* e2 = getenv("PDAE_TC_DBG_BOFF");
-    a.dbg_shift = e1 ? atoi(e1) : 0;
-    a.dbg_boff = e2 ? atoi(e2) : 0;
-  }
   int BN;
   if (head) BN = 16;
   else if (d.bn_override == 64 || d.bn_override == 128 || d.bn_override == 256) BN = d.bn_override;
-  else if (Cout % 256 == 0 && (long long)a.tiles_m * (Cout / 256) >= g_num_sms) BN = 256;  // fewer A re-reads per FLOP
+  // (no automatic BN = 256: its 128 accumulator registers per consumer thread spill; only the softmax GEMM, whose row
+  //  must fit one tile, asks for it)
   else BN = (Cout % 128 == 0) ? 128 : 64;
   if (!head && Cout % BN != 0) {
     delete pl;
@@ -740,7 +634,7 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
   a.tiles_total = a.tiles_m * (head ? 1 : Cout / BN);
   const int b_bytes = ((BN * T2_BK * 2 + 1023) / 1024) * 1024;
   int stage_bytes = T2_A_BYTES + b_bytes;
-  const int staging = head ? 0 : (a.has_res ? 4 : 2) * T2_STG_BYTES;
+  const int staging = head ? 0 : (a.has_res ? 2 : 1) * T2_STG_BYTES;
   const int total_all = a.taps * a.kblocks + a.kblocks2;
   pl->grid = a.tiles_total < g_num_sms ? a.tiles_total : g_num_sms;
   // Weights stationary in shared memory: when the whole layer's B operand fits beside >= 4 A-only stages and every CTA
@@ -906,7 +800,7 @@ extern "C" int pdae_gemm_tc2_create(pdae_conv_tc2_plan** plan_out, const void* a
 }
 
 // P_i = softmax_rows(alpha * A_i * Bm_i^T) stored as bf16: the attention-probability GEMM with the softmax folded into the
-// epilogue (the fp32 score matrix never leaves TMEM).  N must be 64, 128 or 256 (one n-tile holds the whole row).
+// epilogue (the fp32 score matrix never leaves the registers).  N must be 64, 128 or 256 (one n-tile holds the whole row).
 extern "C" int pdae_gemm_tc2_softmax_create(pdae_conv_tc2_plan** plan_out, const void* a_bf16, long long a_ld, long long a_bs,
                                             const void* b_bf16, long long b_ld, long long b_bs, void* out_bf16, long long out_ld,
                                             long long out_bs, int batch, int M, int N, int K, float alpha) {
@@ -926,12 +820,15 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
   PDAE_REQUIRE(pl, "conv_tc2_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
+#define T2_GO(BN, OB) launch_tc2<BN, OB>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s)
+  const bool ob = pl->args.out_bf16 != 0;
   switch (pl->BN) {
-    case 16: e = launch_tc2<16>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s); break;
-    case 64: e = launch_tc2<64>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s); break;
-    case 128: e = launch_tc2<128>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s); break;
-    default: e = launch_tc2<256>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s); break;
+    case 16: e = T2_GO(16, false); break;
+    case 64: e = ob ? T2_GO(64, true) : T2_GO(64, false); break;
+    case 128: e = ob ? T2_GO(128, true) : T2_GO(128, false); break;
+    default: e = ob ? T2_GO(256, true) : T2_GO(256, false); break;
   }
+#undef T2_GO
   if (e != cudaSuccess) {
     (void)cudaGetLastError();
     set_error("launch of conv_tc2_kernel<%d> failed: %s", pl->BN, cudaGetErrorString(e));

@@ -1,37 +1,38 @@
-// conv_tc3 -- 3x3 convolution with the GroupNorm-apply / AdaGN / SiLU prologue FUSED into the operand path (sm_100a).
+// conv_tc3 -- 3x3 convolution with the GroupNorm-apply / AdaGN / SiLU prologue FUSED into the operand path (sm_90a).
 //
 // Reference op chain (model/module.py:278-297, 361-384):   h = conv3x3(SiLU(GN(x)))   and
 // out = conv3x3(SiLU((1+zs)*(GN(h)*(1+s)+sh)+zsh)) [+ skip_1x1(x_raw)] + residual.  The GroupNorm / AdaGN / z-modulation
 // algebra is folded by gn_coef_ch into per-(image, channel) coefficients (a, b); this kernel applies
 // SiLU(a*x + b) while it builds the tensor-core A operand, so the activated tensor never exists in HBM.
 //
-//   warp 17     : TMA producer of the weight (B) tiles                       [tap][Cout][Cin] bf16, SWIZZLE_128B
-//   warp 18     : tcgen05.mma issuer, accumulators double-buffered in TMEM (2 x BN columns)
-//   warps 0-7   : two epilogue groups (one per TMEM accumulator): tcgen05.ld -> +bias (+residual via TMA) -> swizzled
-//                 staging -> per-channel GroupNorm sums (for the NEXT GroupNorm) -> TMA store        (as conv_tc2)
-//   warp 16     : TMA producer of the RAW (pre-normalisation) halo: per 64-channel k-block ONE 4-D box (64 ch x 10 x 18 px,
+//   warp 13     : TMA producer of the weight (B) tiles                       [tap][Cout][Cin] bf16, SWIZZLE_128B
+//   warp 12     : TMA producer of the RAW (pre-normalisation) halo: per 64-channel k-block ONE 4-D box (64 ch x 10 x 18 px,
 //                 out-of-image pixels zero-filled = the conv padding) lands, 128B-swizzled, directly in the operand stage.
-//   warps 8-15  : TRANSFORM group: rewrites that stage IN PLACE, x -> SiLU(a*x+b) (shared memory -> shared memory, no
+//   warps 8-11  : TRANSFORM group: rewrites that stage IN PLACE, x -> SiLU(a*x+b) (shared memory -> shared memory, no
 //                 global-load latency on its path, no extra buffer); padding pixels stay zero.
-// All nine taps of the k-block address that single tile: tap (dy, dx) is the UMMA descriptor started (dy*10 + dx) rows
+//   warps 0-7   : two consumer warpgroups (output rows 0-7 / 8-15 of the 16 x 8 tile): wgmma into fp32 registers, then the
+//                 epilogue from the accumulator fragments: +bias (+residual) -> swizzled staging -> per-channel GroupNorm
+//                 sums (for the NEXT GroupNorm) -> TMA store        (as conv_tc2)
+// All nine taps of the k-block address that single tile: tap (dy, dx) is the wgmma descriptor started (dy*10 + dx) rows
 // into it with a stride-byte-offset of 10 rows (1280 B) between its 8-pixel row groups -- the 128B swizzle is a function
-// of the absolute shared-memory address (scripts/desc_shift_probe.py), so a row-shifted window of a tile written with
-// address-based swizzling is a valid K-major operand.  Shared-memory operand writes per k-block drop from 9 x 16 KB
-// (one TMA box per tap, conv_tc2) to 23 KB, and the separate gn_apply pass over HBM disappears.
+// of the absolute shared-memory address, so a row-shifted window of a tile written with address-based swizzling is a valid
+// K-major operand.  Shared-memory operand writes per k-block drop from 9 x 16 KB (one TMA box per tap, conv_tc2) to 23 KB,
+// and the separate gn_apply pass over HBM disappears.
 //
 // X3 = split-operand mode (fp32-grade products): the source is fp32; the transform writes TWO halo tiles
-// hi = bf16(v), lo = bf16(v - hi); weights come as (W_hi, W_lo) tile pairs; per tap the issuer accumulates
-// a_hi*W_hi + a_lo*W_hi + a_hi*W_lo.  The hi tile is written and read once (conv_tc2's [hi|lo|hi] layout duplicated it).
+// hi = bf16(v), lo = bf16(v - hi); weights come as one merged [W_hi | W_lo] tile; per tap the consumers accumulate
+// a_hi*W_hi + a_hi*W_lo + a_lo*W_hi.
 //
 // The 1x1 skip convolution of a channel-changing ResBlock (model/module.py:268-276) rides along as extra k-blocks whose
 // transform is the identity and whose single tap is the centre window.
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pdae {
 
-constexpr int T3_BM = 128, T3_BK = 64;
+constexpr int T3_BK = 64;
 constexpr int T3_TW = 8, T3_TH = 16;                  // output tile (pixels): 8 wide x 16 tall, one image
 constexpr int T3_P = T3_TW + 2;                       // halo pitch (pixels per halo row)
 constexpr int T3_HROWS = T3_TH + 2;
@@ -39,14 +40,13 @@ constexpr int T3_HALO = T3_P * T3_HROWS;              // 180 halo pixels = 180 s
 constexpr int T3_HALO_BYTES = 23 * 1024;              // 180 * 128 = 23040 B, padded to a 1024-B multiple (swizzle atom alignment)
 constexpr int T3_STG_BYTES = 128 * 128;
 constexpr int T3_MAX_SA = 4, T3_MAX_SB = 12;
-constexpr int T3_XF_WARPS = 8;
-constexpr int T3_THREADS = 64 + 256 + 32 * T3_XF_WARPS + 32 + 32;   // 640: + the raw-halo TMA producer warp + a second MMA issuer
-// Warp roles.  The SM's warp scheduler favours HIGHER warp ids among eligible warps (B300_MICROARCH.md, "hi-wid-first"), so the
-// three single-thread, latency-critical roles get the three highest ids (one per scheduler partition: wid % 4 = 0, 1, 2) and
-// are never starved of issue slots by the 16 compute warps below them.
-constexpr int T3_W_RAWPROD = 16, T3_W_BPROD = 17, T3_W_MMA = 18;   // warps 0-7: two epilogue groups, 8-15: transform group
-constexpr int T3_W_MMA2 = 19;                                      // second MMA issuer (DU variants), idle otherwise
-constexpr int T3_XF_PASSES = (T3_HALO + 31) / 32;     // 6 passes of 32 pixel slots (8 threads x 16 B per pixel)
+constexpr int T3_XF_WARPS = 4;
+// 448 threads = 14 warps: at most 4 warps per scheduler partition, so each thread may hold 128 registers (the consumers keep
+// BN / 2 fp32 accumulators each).
+constexpr int T3_THREADS = 256 + 32 * T3_XF_WARPS + 32 + 32;
+constexpr int T3_W_RAWPROD = 8 + T3_XF_WARPS, T3_W_BPROD = 9 + T3_XF_WARPS;   // warps 0-7: consumers, 8-11: transform group
+constexpr int T3_XF_SLOTS = 4 * T3_XF_WARPS;                                  // pixel slots per pass (8 threads x 16 B per pixel)
+constexpr int T3_XF_PASSES = (T3_HALO + T3_XF_SLOTS - 1) / T3_XF_SLOTS;     // 12 passes of 16 pixel slots
 
 struct ConvTc3Args {
   int C1, C2;                           // pre-activation conv input = virtual channel concat C1 | C2 (tensor maps tmS1 | tmS2)
@@ -60,8 +60,6 @@ struct ConvTc3Args {
   int kblocks, kblocks2;
   int sa, sb;                           // pipeline depths: halo stages / weight-tile stages
   int has_res, out_bf16, silu;
-  int dbg_mode;                         // timing experiments only (wrong results): 1 = aligned start + dense SBO, 2 = dense SBO, 3 = aligned start
-  unsigned long long* dbg;              // tuning aid (PDAE_TC3_DBG=1): per-role wait-cycle counters, nullptr in production
 };
 
 // ---- small PTX helpers (same protocol as conv_tc2.cu) -------------------------------------------------------------------
@@ -88,9 +86,8 @@ __device__ __forceinline__ uint32_t mb_try(uint32_t bar, uint32_t parity) {
   return done;
 }
 // Slow path of a wait: mbarrier.try_wait with a SUSPEND-TIME HINT, so a waiting warp sleeps in hardware (it is woken by the
-// completing arrive) instead of re-issuing the poll every ~100 cycles.  With 18+ warps per CTA of which most are waiting at
-// any time, hot polling took more than half of all issue slots away from the warps that had work (ncu: 8.4 M polls per
-// launch, profiles/r02_ncu_conv_tc3_spin.txt).
+// completing arrive) instead of re-issuing the poll: most of the CTA's warps are waiting at any time, and hot polling takes
+// issue slots away from the warps that have work.
 __device__ __forceinline__ uint32_t mb_try_sleep(uint32_t bar, uint32_t parity) {
   uint32_t done;
   asm volatile(
@@ -111,16 +108,6 @@ __device__ __forceinline__ void mb_wait(uint32_t bar, uint32_t parity) {
   if (mb_try(bar, parity)) return;   // fast path: already complete
   mb_wait_slow(bar, parity);
 }
-// wait that also accumulates the cycles spent into *acc when profiling is on
-__device__ __forceinline__ void mb_wait_t(uint32_t bar, uint32_t parity, unsigned long long* dbg, unsigned long long& acc) {
-  if (dbg) {
-    const long long t0 = clock64();
-    mb_wait(bar, parity);
-    acc += (unsigned long long)(clock64() - t0);
-  } else {
-    mb_wait(bar, parity);
-  }
-}
 __device__ __forceinline__ void tma_ld4(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3) {
   asm volatile(
       "cp.async.bulk.tensor.4d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6}], [%2];"
@@ -138,42 +125,15 @@ __device__ __forceinline__ void tma_st4(const CUtensorMap* m, uint32_t src, int 
                "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
-// K-major SWIZZLE_128B operand descriptor; sbo = bytes between consecutive 8-row groups
-__device__ __forceinline__ uint64_t sw128_desc(uint32_t saddr, uint32_t sbo) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | (1ull << 16) | ((uint64_t)(sbo >> 4) << 32) | (1ull << 46) | (2ull << 61);
-}
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(a), "l"(b), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_to(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
-// One elected lane of a fully converged warp.  The issuer / producer loops are executed by ALL 32 lanes (warp-uniform control
-// flow and operands, which the compiler keeps in uniform registers); only the tcgen05 / TMA instruction itself is predicated on
-// the elected lane.  Running the loop under `if (lane == 0)` instead made every descriptor a per-lane value: each MMA then cost
-// an ELECT + 5 x R2UR.BROADCAST + branch 'waterfall' (~200 cycles of issue per MMA, profiles/r02_ncu_conv_tc3_spin.txt).
+// One elected lane of a fully converged warp.  The producer loops are executed by ALL 32 lanes (warp-uniform control flow and
+// operands, which the compiler keeps in uniform registers); only the TMA instruction itself is predicated on the elected lane.
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
 }
-__device__ __forceinline__ void epi_bar(int g) { asm volatile("bar.sync %0, 128;" ::"r"(1 + g) : "memory"); }
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
-}
+// barrier of the 256 consumer threads (the other warps never join it)
+__device__ __forceinline__ void cons_bar() { asm volatile("bar.sync 1, 256;" ::: "memory"); }
 // byte offset of (row, 16-byte chunk) inside a SWIZZLE_128B tile whose base is 1024-B aligned
 __device__ __forceinline__ uint32_t swz(int row, int chunk16) { return (uint32_t)(row * 128 + ((chunk16 ^ (row & 7)) << 4)); }
 
@@ -194,7 +154,7 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 }
 }  // namespace t3
 
-template <int BN, bool X3, bool MG = true, bool DU = false>
+template <int BN, bool X3, bool OB>
 __global__ void __launch_bounds__(T3_THREADS, 1)
 conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmB2,
                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
@@ -204,33 +164,23 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_a_full[T3_MAX_SA], bar_a_empty[T3_MAX_SA], bar_raw[T3_MAX_SA];
   __shared__ __align__(8) uint64_t bar_b_full[T3_MAX_SB], bar_b_empty[T3_MAX_SB];
-  __shared__ __align__(8) uint64_t bar_acc_full[2], bar_acc_empty[2], bar_res[2];
-  __shared__ uint32_t tmem_slot;
-  __shared__ float st_acc[2][2][BN];   // [epilogue group][sum | sum^2][channel] of the group's current (image, n-tile)
+  __shared__ __align__(8) uint64_t bar_res;
+  __shared__ float st_acc[2][BN];   // [sum | sum^2][channel] of the current (image, n-tile)
+  __shared__ float st_part[2][256]; // per-chunk partial sums [sum | sum^2][row run * CW + column]
 
-  // Split mode: W_hi and W_lo of a (tap, k-block) arrive as ONE 2*BN-row tile [W_hi | W_lo]; the issuer runs
-  // a_hi x [W_hi | W_lo] as a single N = 2*BN MMA (accumulator columns 0..BN-1: hi*hi, BN..2BN-1: hi*lo) and a_lo x W_hi as an
-  // N = BN MMA into columns 0..BN-1; the epilogue adds the two halves.  8 instead of 12 MMAs per tap and a third less operand
-  // traffic -- the 64/128-wide layers are bound by the shared-memory port (the A tile is re-read per MMA), not the tensor pipe.
-  // (MG = false keeps the unmerged BN = 128 schedule for A/B measurements, PDAE_TC3_MRG128=0.)
-  constexpr bool MRG = X3 && (BN == 64 || MG);
-  // DU (experimental, opt-in -- see pdae_conv_tc3_create): TWO MMA-issuer warps take alternate taps and accumulate into separate TMEM blocks (the epilogue adds them).  One
-  // issuer spends ~100 cycles of uniform-datapath work per MMA (descriptor arithmetic, barrier polls, commit) -- more than a
-  // 64- or 128-wide MMA occupies the tensor pipe -- so the narrow layers are issue-bound with a single issuer.
-  constexpr int ACC1 = MRG ? 2 * BN : BN;                       // accumulator columns of one issuer
-  constexpr bool DUAL = DU && (!X3 || MRG) && 4 * ACC1 <= 512;  // one weight stage per tap, both blocks double-buffered
-  constexpr int ACC_COLS = (DUAL ? 2 : 1) * ACC1;
-  constexpr int B_BYTES = (MRG ? 2 * BN : BN) * T3_BK * 2;
+  // Split mode: W_hi and W_lo of a (tap, k-block) arrive as ONE 2*BN-row tile [W_hi | W_lo]; per k-step the consumers run
+  // a_hi x W_hi, a_hi x W_lo and a_lo x W_hi into the same accumulators.
+  constexpr int B_BYTES = (X3 ? 2 * BN : BN) * T3_BK * 2;
   constexpr int A_STAGE = (X3 ? 2 : 1) * T3_HALO_BYTES;
-  constexpr int TMEM_COLS = 2 * ACC_COLS;
-  constexpr int NMAT = (X3 && !MRG) ? 2 : 1;   // weight tiles per (tap, k-block): W | (W_hi, W_lo) | merged [W_hi | W_lo]
-  constexpr int ZMUL = X3 ? 2 : 1;             // weight matrices per tap in global memory
+  constexpr int CW = OB ? 64 : 32;             // accumulator columns per staging tile (128-byte rows)
+  constexpr int NCH = BN / CW;
+  constexpr int RPT = CW / 2;                  // statistics: rows per thread (256 threads = CW columns x 128 / RPT row runs)
   const uint32_t smem0 = (s_u32(smem_raw) + 1023u) & ~1023u;
   const int SA = p.sa, SB = p.sb;
   const uint32_t a_base = smem0;
   const uint32_t b_base = a_base + (uint32_t)(SA * A_STAGE);
   const uint32_t stg_out = b_base + (uint32_t)(SB * B_BYTES);
-  const uint32_t stg_res = stg_out + 2u * T3_STG_BYTES;
+  const uint32_t stg_res = stg_out + (uint32_t)T3_STG_BYTES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int total_it = p.kblocks + p.kblocks2;
   const int per_cta = (p.tiles_total + (int)gridDim.x - 1) / (int)gridDim.x;
@@ -239,157 +189,51 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
   const int tiles_img = p.tiles_x * p.tiles_y;
 
   for (int j = threadIdx.x; j < BN; j += T3_THREADS) {
-    st_acc[0][0][j] = 0.f; st_acc[0][1][j] = 0.f;
-    st_acc[1][0][j] = 0.f; st_acc[1][1][j] = 0.f;
+    st_acc[0][j] = 0.f;
+    st_acc[1][j] = 0.f;
   }
   if (threadIdx.x == 0) {
     for (int s = 0; s < SA; ++s) {
       mb_init(s_u32(&bar_a_full[s]), T3_XF_WARPS);   // one elected arrive per transform warp
-      mb_init(s_u32(&bar_a_empty[s]), DUAL ? 2 : 1);     // every issuer commits once per k-block
+      mb_init(s_u32(&bar_a_empty[s]), 8);            // one arrive per consumer warp
       mb_init(s_u32(&bar_raw[s]), 1);
     }
     for (int s = 0; s < SB; ++s) {
       mb_init(s_u32(&bar_b_full[s]), 1);
-      mb_init(s_u32(&bar_b_empty[s]), 1);
+      mb_init(s_u32(&bar_b_empty[s]), 8);
     }
-    for (int i = 0; i < 2; ++i) {
-      mb_init(s_u32(&bar_acc_full[i]), DUAL ? 2 : 1);
-      mb_init(s_u32(&bar_acc_empty[i]), 1);
-      mb_init(s_u32(&bar_res[i]), 1);
-    }
+    mb_init(s_u32(&bar_res), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmO) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmS1) : "memory");
   }
-  if (warp == T3_W_MMA) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(&tmem_slot)), "n"(TMEM_COLS)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_slot;
 
   if (warp == T3_W_BPROD) {
     // ================= weight-tile TMA producer (warp-uniform loop, elected lane issues) =================
     int s = 0;
     uint32_t ph = 0;
-    unsigned long long w_b = 0;
     for (int tile = tile_begin; tile < tile_end; ++tile) {
       const int n0 = (tile / p.tiles_m) * BN;
       for (int it = 0; it < total_it; ++it) {
         const bool skipk = it >= p.kblocks;
         const int ntap = skipk ? 1 : 9;
         for (int tap = 0; tap < ntap; ++tap) {
-#pragma unroll
-          for (int m = 0; m < NMAT; ++m) {
-            mb_wait_t(s_u32(&bar_b_empty[s]), ph ^ 1u, p.dbg, w_b);
-            const uint32_t full = s_u32(&bar_b_full[s]);
-            const uint32_t dst = b_base + (uint32_t)(s * B_BYTES);
-            if (elect_one()) {
-              mb_expect_tx(full, (uint32_t)B_BYTES);
-              if (!skipk) tma_ld3(dst, &tmB, full, it * T3_BK, n0, tap * ZMUL + m);
-              else tma_ld3(dst, &tmB2, full, (it - p.kblocks) * T3_BK, n0, m);
-            }
-            __syncwarp();
-            if (++s == SB) { s = 0; ph ^= 1u; }
-          }
-        }
-      }
-    }
-    if (p.dbg && lane == 0) atomicAdd(p.dbg + 4, w_b);
-  } else if (warp == T3_W_MMA || (DUAL && warp == T3_W_MMA2)) {
-    // ================= MMA issuer(s) (warp-uniform loop, elected lane issues) =================
-    constexpr uint32_t IDESC =
-        (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)(BN >> 3) << 17) | ((uint32_t)(T3_BM >> 4) << 24);
-    constexpr uint32_t A_SBO = (uint32_t)T3_P * 128u;   // 8-pixel row groups of the halo are one halo row (10 px) apart
-    const uint32_t tmem_u = __shfl_sync(0xffffffffu, tmem_base, 0);
-    const int wi = warp - T3_W_MMA;                     // issuer index: takes the taps with (running tap count & 1) == wi
-    int sa = 0, sb = 0, tl = 0;
-    uint32_t pha = 0, phb = 0, g = 0;
-    unsigned long long w_a = 0, w_bf = 0, w_acc = 0;
-    for (int tile = tile_begin; tile < tile_end; ++tile, ++tl) {
-      const int ab = tl & 1;
-      mb_wait_t(s_u32(&bar_acc_empty[ab]), (uint32_t)(((tl >> 1) & 1) ^ 1), p.dbg, w_acc);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t tmem_d = tmem_u + (uint32_t)(ab * ACC_COLS + (DUAL ? wi * ACC1 : 0));
-      uint32_t started = 0;                             // 0 until this issuer's first MMA of the tile (which overwrites)
-      for (int it = 0; it < total_it; ++it) {
-        mb_wait_t(s_u32(&bar_a_full[sa]), pha, p.dbg, w_a);
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        const bool skipk = it >= p.kblocks;
-        const int ntap = skipk ? 1 : 9;
-        const uint32_t a_hi = a_base + (uint32_t)(sa * A_STAGE);
-        int ty3 = skipk ? 1 : 0, tx3 = skipk ? 1 : 0;    // tap = (ty3, tx3); the 1x1 skip conv reads the centre tap
-        for (int tp = 0; tp < ntap; ++tp, ++g) {
-          const uint32_t off = (uint32_t)(ty3 * T3_P + tx3) * 128u;
-          if (++tx3 == 3) { tx3 = 0; ++ty3; }
-          if (DUAL && (int)(g & 1u) != wi) {             // the other issuer's tap: only keep the stage ring in step
-            if (++sb == SB) { sb = 0; phb ^= 1u; }
-            continue;
-          }
-          const uint64_t ad_hi = sw128_desc(a_hi + off, A_SBO);
-          mb_wait_t(s_u32(&bar_b_full[sb]), phb, p.dbg, w_bf);
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-          const uint64_t bd = sw128_desc(b_base + (uint32_t)(sb * B_BYTES), 1024u);
-          const uint32_t first = started;
-          started = 1u;
-          const uint32_t bar_be = s_u32(&bar_b_empty[sb]);
-          if (MRG) {
-            constexpr uint32_t IDESC128 =
-                (1u << 4) | (1u << 7) | (1u << 10) | ((uint32_t)((2 * BN) >> 3) << 17) | ((uint32_t)(T3_BM >> 4) << 24);
-            if (elect_one()) {
-              const uint64_t ad_lo = sw128_desc(a_hi + (uint32_t)T3_HALO_BYTES + off, A_SBO);
-              umma(tmem_d, ad_hi, bd, IDESC128, first);                                   // a_hi x [W_hi | W_lo]
-#pragma unroll
-              for (int k = 1; k < T3_BK / 16; ++k) umma(tmem_d, ad_hi + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), IDESC128, 1u);
-#pragma unroll
-              for (int k = 0; k < T3_BK / 16; ++k) umma(tmem_d, ad_lo + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), IDESC, 1u);   // a_lo x W_hi
-              umma_commit_to(bar_be);
-            }
-            __syncwarp();
-            if (++sb == SB) { sb = 0; phb ^= 1u; }
-            continue;
-          }
+          mb_wait(s_u32(&bar_b_empty[s]), ph ^ 1u);
+          const uint32_t full = s_u32(&bar_b_full[s]);
+          const uint32_t dst = b_base + (uint32_t)(s * B_BYTES);
           if (elect_one()) {
-            umma(tmem_d, ad_hi, bd, IDESC, first);
-#pragma unroll
-            for (int k = 1; k < T3_BK / 16; ++k) umma(tmem_d, ad_hi + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), IDESC, 1u);
-            if (X3) {
-              const uint64_t ad_lo = sw128_desc(a_hi + (uint32_t)T3_HALO_BYTES + off, A_SBO);
-#pragma unroll
-              for (int k = 0; k < T3_BK / 16; ++k) umma(tmem_d, ad_lo + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), IDESC, 1u);
-            }
-            umma_commit_to(bar_be);
+            mb_expect_tx(full, (uint32_t)B_BYTES);
+            if (!skipk) tma_ld3(dst, &tmB, full, it * T3_BK, n0, tap * (X3 ? 2 : 1));
+            else tma_ld3(dst, &tmB2, full, (it - p.kblocks) * T3_BK, n0, 0);
           }
           __syncwarp();
-          if (++sb == SB) { sb = 0; phb ^= 1u; }
-          if (X3) {   // a_hi * W_lo
-            mb_wait(s_u32(&bar_b_full[sb]), phb);
-            asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-            const uint64_t bd2 = sw128_desc(b_base + (uint32_t)(sb * B_BYTES), 1024u);
-            const uint32_t bar_be2 = s_u32(&bar_b_empty[sb]);
-            if (elect_one()) {
-#pragma unroll
-              for (int k = 0; k < T3_BK / 16; ++k) umma(tmem_d, ad_hi + (uint64_t)(2 * k), bd2 + (uint64_t)(2 * k), IDESC, 1u);
-              umma_commit_to(bar_be2);
-            }
-            __syncwarp();
-            if (++sb == SB) { sb = 0; phb ^= 1u; }
-          }
+          if (++s == SB) { s = 0; ph ^= 1u; }
         }
-        if (elect_one()) umma_commit_to(s_u32(&bar_a_empty[sa]));
-        __syncwarp();
-        if (++sa == SA) { sa = 0; pha ^= 1u; }
       }
-      if (elect_one()) umma_commit_to(s_u32(&bar_acc_full[ab]));
-      __syncwarp();
     }
-    if (p.dbg && lane == 0 && wi == 0) { atomicAdd(p.dbg + 0, w_a); atomicAdd(p.dbg + 1, w_bf); atomicAdd(p.dbg + 2, w_acc); }
   } else if (warp == T3_W_RAWPROD) {
     // ================= raw-halo TMA producer (warp-uniform loop, elected lane issues) =================
     // item (tile, k-block) -> ONE box of the pre-activation tensor: 64 channels x 10 x 18 pixels starting one pixel up-left of
@@ -398,7 +242,6 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
     constexpr uint32_t RAW_TX = (uint32_t)(T3_HALO * 128 * (X3 ? 2 : 1));
     int s = 0;
     uint32_t ph = 0;
-    unsigned long long w_r = 0;
     for (int tile = tile_begin; tile < tile_end; ++tile) {
       int mt = tile % p.tiles_m;
       const int tx = mt % p.tiles_x;
@@ -416,7 +259,7 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
           const int kc = (it - p.kblocks) * T3_BK;
           if (kc < p.S1) { m = &tmK1; c0 = kc; } else { m = &tmK2; c0 = kc - p.S1; }
         }
-        mb_wait_t(s_u32(&bar_a_empty[s]), ph ^ 1u, p.dbg, w_r);
+        mb_wait(s_u32(&bar_a_empty[s]), ph ^ 1u);
         const uint32_t full = s_u32(&bar_raw[s]);
         const uint32_t dst = a_base + (uint32_t)(s * A_STAGE);
         if (elect_one()) {
@@ -428,16 +271,13 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
         if (++s == SA) { s = 0; ph ^= 1u; }
       }
     }
-    if (p.dbg && lane == 0) atomicAdd(p.dbg + 3, w_r);
   } else if (warp >= 8 && warp < 8 + T3_XF_WARPS) {
     // ================= transform group: raw halo (in the operand stage) -> SiLU(a*x+b) [-> hi | lo], IN PLACE =================
-    const int tt = (int)threadIdx.x - 256;   // 0..255
-    const int slot = tt >> 3, ch8 = tt & 7;  // pixel slot (32 per pass), 8-channel chunk (16 B of bf16 operand)
+    const int tt = (int)threadIdx.x - 256;   // 0..T3_XF_SLOTS*8-1
+    const int slot = tt >> 3, ch8 = tt & 7;  // pixel slot (T3_XF_SLOTS per pass), 8-channel chunk (16 B of bf16 operand)
     const int C = p.C1 + p.C2;
     int s = 0;
     uint32_t ph = 0;
-    unsigned long long w_x = 0;
-    const long long t_begin = p.dbg ? clock64() : 0;
     for (int tile = tile_begin; tile < tile_end; ++tile) {
       int mt = tile % p.tiles_m;
       const int tx = mt % p.tiles_x;
@@ -449,7 +289,7 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
       uint32_t inimg = 0, interior = 0;
 #pragma unroll
       for (int j = 0; j < T3_XF_PASSES; ++j) {
-        const int hp = j * 32 + slot;
+        const int hp = j * T3_XF_SLOTS + slot;
         const int hy = hp / T3_P, hx = hp - hy * T3_P;
         const int gy = y0 + hy, gx = x0 + hx;
         if (hp < T3_HALO && gy >= 0 && gy < p.H && gx >= 0 && gx < p.W) {
@@ -471,7 +311,7 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
           for (int j = 0; j < 8; ++j) { ca[j] = 1.f; cb[j] = 0.f; }
         }
         const int silu = skipk ? 0 : p.silu;
-        mb_wait_t(s_u32(&bar_raw[s]), ph, p.dbg, w_x);
+        mb_wait(s_u32(&bar_raw[s]), ph);
         const uint32_t hi_base = a_base + (uint32_t)(s * A_STAGE);
         // bf16 mode: the raw input of the 1x1 skip conv IS the operand -- nothing to do.  Split mode: it still needs the hi/lo
         // split, but only where the centre tap reads it.
@@ -479,7 +319,7 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
 #pragma unroll
         for (int j = 0; j < T3_XF_PASSES; ++j) {
           if (todo & (1u << j)) {
-            const int hp = j * 32 + slot;
+            const int hp = j * T3_XF_SLOTS + slot;
             float v[8];
             if (X3) {
               // raw fp32: channels 0-31 of the k-block sit in the hi region, 32-63 in the lo region (128-B swizzled rows)
@@ -530,22 +370,23 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
         if (++s == SA) { s = 0; ph ^= 1u; }
       }
     }
-    if (p.dbg && tt == 0) { atomicAdd(p.dbg + 5, w_x); atomicAdd(p.dbg + 6, (unsigned long long)(clock64() - t_begin)); }
   } else if (warp < 8) {
-    // ================= epilogue: two groups of 128 threads; group g drains accumulator buffer g (as conv_tc2) =================
-    const int eg = warp >> 2;
-    const int et = (int)threadIdx.x - eg * 128;
-    const bool elected = et == 0;
-    const int q = warp & 3;                    // TMEM lane quadrant of this warp
-    const int r = q * 32 + lane;               // accumulator row = pixel index in the tile (row-major 16 x 8)
+    // ================= consumers: warpgroup wg computes output rows [8 wg, 8 wg + 8) of the 16 x 8 tile, then both run the
+    // epilogue straight from the accumulator fragments (as conv_tc2) =================
+    constexpr uint32_t A_SBO = (uint32_t)T3_P * 128u;   // 8-pixel row groups of the halo are one halo row (10 px) apart
+    const int wg = warp >> 2;
+    const int t = threadIdx.x & 127;
+    const int ct = threadIdx.x;                // 0..255
+    const bool elected = ct == 0;
     int rc = 0;
-    unsigned long long w_e = 0;
-    const long long te_begin = p.dbg ? clock64() : 0;
-    const uint32_t obuf = stg_out + (uint32_t)eg * T3_STG_BYTES, rbuf = stg_res + (uint32_t)eg * T3_STG_BYTES;
-    const uint32_t rbar = s_u32(&bar_res[eg]);
-    const int CW = p.out_bf16 ? 64 : 32;       // accumulator columns per staging tile (128-byte rows)
-    const int nch = BN / CW;
-    for (int tile = tile_begin + eg, tl = eg; tile < tile_end; tile += 2, tl += 2) {
+    int sa = 0, sb = 0;
+    uint32_t pha = 0, phb = 0;
+    const uint32_t obuf = stg_out, rbuf = stg_res;
+    const uint32_t rbar = s_u32(&bar_res);
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    for (int tile = tile_begin; tile < tile_end; ++tile) {
       const int nt = tile / p.tiles_m;
       int mt = tile - nt * p.tiles_m;
       const int tx = mt % p.tiles_x;
@@ -553,182 +394,179 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
       const int ty = mt % p.tiles_y;
       const int b0 = mt / p.tiles_y;
       const int x0 = tx * T3_TW, y0 = ty * T3_TH, n0 = nt * BN;
-      const int ab = tl & 1;
-      const uint32_t tmem_acc = tmem_base + (uint32_t)(ab * ACC_COLS) + ((uint32_t)(q * 32) << 16);
-      if (!X3 && p.has_res && elected) {       // residual chunk 0 (issued before the accumulator is needed)
+      if (!X3 && p.has_res && elected) {       // residual chunk 0 (lands while the main loop runs)
         mb_expect_tx(rbar, T3_STG_BYTES);
         tma_ld4(rbuf, &tmR, rbar, n0, x0, y0, b0);
       }
-      mb_wait_t(s_u32(&bar_acc_full[ab]), (uint32_t)((tl >> 1) & 1), p.dbg, w_e);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      for (int c = 0; c < nch; ++c) {
-        float val[64];
-        {
-          uint32_t v[32];
-          tmem_ld32(tmem_acc + (uint32_t)(c * CW), v);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+      // ---- main loop: per k-block one halo stage, per tap one weight stage; a weight stage is released once the MMAs
+      // reading it have retired, the halo stage at the end of its k-block ----
+      uint32_t started = 0;                    // 0 until the tile's first MMA (which overwrites)
+      int pend_b = -1;
+      for (int it = 0; it < total_it; ++it) {
+        mb_wait(s_u32(&bar_a_full[sa]), pha);
+        const bool skipk = it >= p.kblocks;
+        const int ntap = skipk ? 1 : 9;
+        const uint32_t a_hi = a_base + (uint32_t)(sa * A_STAGE) + (uint32_t)wg * (8u * A_SBO);
+        int ty3 = skipk ? 1 : 0, tx3 = skipk ? 1 : 0;    // tap = (ty3, tx3); the 1x1 skip conv reads the centre tap
+        for (int tp = 0; tp < ntap; ++tp) {
+          const uint32_t off = (uint32_t)(ty3 * T3_P + tx3) * 128u;
+          if (++tx3 == 3) { tx3 = 0; ++ty3; }
+          const uint64_t ad_hi = wgmma::desc_sw128(a_hi + off, 16u, A_SBO);
+          mb_wait(s_u32(&bar_b_full[sb]), phb);
+          const uint64_t bd = wgmma::desc_sw128(b_base + (uint32_t)(sb * B_BYTES), 16u, 1024u);
+          wgmma::fence();
 #pragma unroll
-          for (int j = 0; j < 32; ++j) val[j] = __uint_as_float(v[j]);
-          if (MRG) {   // + the a_hi x W_lo half of the merged accumulator (split mode stores fp32: CW = 32)
-            tmem_ld32(tmem_acc + (uint32_t)(BN + c * CW), v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
+          for (int k = 0; k < T3_BK / 16; ++k)
+            wgmma::mma<BN, 0>(acc, ad_hi + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), started | (uint32_t)(k != 0));
+          if (X3) {
+            const uint64_t ad_lo = wgmma::desc_sw128(a_hi + (uint32_t)T3_HALO_BYTES + off, 16u, A_SBO);
+            const uint64_t bd_lo = bd + (uint64_t)((BN * 128) >> 4);   // W_lo: the second BN rows of the merged tile
 #pragma unroll
-            for (int j = 0; j < 32; ++j) val[j] += __uint_as_float(v[j]);
-          }
-          if (DUAL) {  // + the second issuer's block
-            tmem_ld32(tmem_acc + (uint32_t)(ACC1 + c * CW), v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int j = 0; j < 32; ++j) val[j] += __uint_as_float(v[j]);
-            if (MRG) {
-              tmem_ld32(tmem_acc + (uint32_t)(ACC1 + BN + c * CW), v);
-              asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-              for (int j = 0; j < 32; ++j) val[j] += __uint_as_float(v[j]);
+            for (int k = 0; k < T3_BK / 16; ++k) {
+              wgmma::mma<BN, 0>(acc, ad_hi + (uint64_t)(2 * k), bd_lo + (uint64_t)(2 * k), 1u);   // a_hi x W_lo
+              wgmma::mma<BN, 0>(acc, ad_lo + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), 1u);      // a_lo x W_hi
             }
           }
-          if (p.out_bf16) {
-            tmem_ld32(tmem_acc + (uint32_t)(c * CW + 32), v);
-            asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-            for (int j = 0; j < 32; ++j) val[32 + j] = __uint_as_float(v[j]);
-            if (DUAL) {
-              tmem_ld32(tmem_acc + (uint32_t)(ACC1 + c * CW + 32), v);
-              asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-              for (int j = 0; j < 32; ++j) val[32 + j] += __uint_as_float(v[j]);
-            }
-          }
+          wgmma::commit();
+          started = 1u;
+          wgmma::wait<1>();
+          if (pend_b >= 0 && lane == 0) mb_arrive(s_u32(&bar_b_empty[pend_b]));
+          pend_b = sb;
+          if (++sb == SB) { sb = 0; phb ^= 1u; }
         }
-        if (p.bias) {
-          const float4* bp = reinterpret_cast<const float4*>(p.bias + n0 + c * CW);
+        wgmma::wait<0>();
+        if (lane == 0) {
+          mb_arrive(s_u32(&bar_b_empty[pend_b]));
+          mb_arrive(s_u32(&bar_a_empty[sa]));
+        }
+        pend_b = -1;
+        if (++sa == SA) { sa = 0; pha ^= 1u; }
+      }
+
 #pragma unroll
-          for (int j = 0; j < 16; ++j) {
-            if (j * 4 < CW) {
-              const float4 bv = __ldg(bp + j);
-              val[4 * j + 0] += bv.x; val[4 * j + 1] += bv.y; val[4 * j + 2] += bv.z; val[4 * j + 3] += bv.w;
-            }
+      for (int c = 0; c < NCH; ++c) {
+        float v[CW / 2];
+#pragma unroll
+        for (int q = 0; q < CW / 2; ++q) v[q] = acc[c * (CW / 2) + q];
+        if (p.bias) {
+#pragma unroll
+          for (int q = 0; q < CW / 2; q += 2) {
+            const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + n0 + c * CW + wgmma::frag_col(t, q)));
+            v[q] += bv.x; v[q + 1] += bv.y;
           }
         }
         if (X3 && p.has_res) {
-          // split mode: the fp32 residual row of this pixel (32 channels = one 128-B line) comes straight from global memory
-          // -- no shared-memory staging, which leaves room for a deeper weight pipeline
-          const float4* rp = reinterpret_cast<const float4*>(
-              p.res_f32 + (((long long)b0 * p.H + y0 + (r >> 3)) * p.W + x0 + (r & 7)) * p.Cout + n0 + c * CW);
+          // split mode: the fp32 residual comes straight from global memory -- no shared-memory staging, which leaves room
+          // for a deeper weight pipeline
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            const float4 rv = __ldg(rp + j);
-            val[4 * j + 0] += rv.x; val[4 * j + 1] += rv.y; val[4 * j + 2] += rv.z; val[4 * j + 3] += rv.w;
+          for (int q = 0; q < CW / 2; q += 2) {
+            const int r = 64 * wg + wgmma::frag_row(t, q);
+            const float2 rv = __ldg(reinterpret_cast<const float2*>(
+                p.res_f32 + (((long long)b0 * p.H + y0 + (r >> 3)) * p.W + x0 + (r & 7)) * p.Cout + n0 + c * CW + wgmma::frag_col(t, q)));
+            v[q] += rv.x; v[q + 1] += rv.y;
           }
         }
         if (!X3 && p.has_res) {
           mb_wait(rbar, (uint32_t)(rc & 1));
-          if (p.out_bf16) {
 #pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              uint32_t w[4];
-              asm volatile("ld.shared.v4.b32 {%0,%1,%2,%3}, [%4];" : "=r"(w[0]), "=r"(w[1]), "=r"(w[2]), "=r"(w[3])
-                           : "r"(rbuf + swz(r, j)));
-#pragma unroll
-              for (int h = 0; h < 4; ++h) {
-                val[8 * j + 2 * h] += __uint_as_float(w[h] << 16);
-                val[8 * j + 2 * h + 1] += __uint_as_float(w[h] & 0xffff0000u);
-              }
-            }
-          } else {
-#pragma unroll
-            for (int j = 0; j < 8; ++j) {
-              float4 rv;
-              asm volatile("ld.shared.v4.f32 {%0,%1,%2,%3}, [%4];" : "=f"(rv.x), "=f"(rv.y), "=f"(rv.z), "=f"(rv.w)
-                           : "r"(rbuf + swz(r, j)));
-              val[4 * j + 0] += rv.x; val[4 * j + 1] += rv.y; val[4 * j + 2] += rv.z; val[4 * j + 3] += rv.w;
+          for (int q = 0; q < CW / 2; q += 2) {
+            const int r = 64 * wg + wgmma::frag_row(t, q), cl = wgmma::frag_col(t, q);
+            if (OB) {
+              uint32_t w;
+              asm volatile("ld.shared.b32 %0, [%1];" : "=r"(w) : "r"(rbuf + swz(r, cl >> 3) + (uint32_t)((cl & 7) * 2)));
+              v[q] += __uint_as_float(w << 16);
+              v[q + 1] += __uint_as_float(w & 0xffff0000u);
+            } else {
+              float2 rv;
+              asm volatile("ld.shared.v2.f32 {%0,%1}, [%2];" : "=f"(rv.x), "=f"(rv.y)
+                           : "r"(rbuf + swz(r, cl >> 2) + (uint32_t)((cl & 3) * 4)));
+              v[q] += rv.x; v[q + 1] += rv.y;
             }
           }
           ++rc;
         }
         if (elected) asm volatile("cp.async.bulk.wait_group.read 0;" ::: "memory");   // previous TMA store has read the staging buffer
-        epi_bar(eg);
-        if (!X3 && p.has_res && elected && c + 1 < nch) {
+        cons_bar();
+        if (!X3 && p.has_res && elected && c + 1 < NCH) {
           mb_expect_tx(rbar, T3_STG_BYTES);
           tma_ld4(rbuf, &tmR, rbar, n0 + (c + 1) * CW, x0, y0, b0);
         }
-        if (p.out_bf16) {
 #pragma unroll
-          for (int j = 0; j < 8; ++j) {
-            uint32_t w[4];
-#pragma unroll
-            for (int h = 0; h < 4; ++h) w[h] = pack_bf16(val[8 * j + 2 * h], val[8 * j + 2 * h + 1]);
-            asm volatile("st.shared.v4.b32 [%0], {%1,%2,%3,%4};" ::"r"(obuf + swz(r, j)), "r"(w[0]), "r"(w[1]), "r"(w[2]), "r"(w[3])
+        for (int q = 0; q < CW / 2; q += 2) {
+          const int r = 64 * wg + wgmma::frag_row(t, q), cl = wgmma::frag_col(t, q);
+          if (OB) {
+            asm volatile("st.shared.b32 [%0], %1;" ::"r"(obuf + swz(r, cl >> 3) + (uint32_t)((cl & 7) * 2)),
+                         "r"(pack_bf16(v[q], v[q + 1]))
+                         : "memory");
+          } else {
+            asm volatile("st.shared.v2.f32 [%0], {%1,%2};" ::"r"(obuf + swz(r, cl >> 2) + (uint32_t)((cl & 3) * 4)), "f"(v[q]),
+                         "f"(v[q + 1])
                          : "memory");
           }
-        } else {
-#pragma unroll
-          for (int j = 0; j < 8; ++j)
-            asm volatile("st.shared.v4.f32 [%0], {%1,%2,%3,%4};" ::"r"(obuf + swz(r, j)), "f"(val[4 * j]), "f"(val[4 * j + 1]),
-                         "f"(val[4 * j + 2]), "f"(val[4 * j + 3])
-                         : "memory");
         }
         asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
-        epi_bar(eg);
+        cons_bar();
         if (elected) {
           tma_st4(&tmO, obuf, n0 + c * CW, x0, y0, b0);
           asm volatile("cp.async.bulk.commit_group;" ::: "memory");
         }
         if (p.ch_stats) {
           // per-channel partial sums over this tile's rows, read back from the staged (rounded) values:
-          // thread -> column (et % CW), rows [(et / CW) * CW, +CW); accumulated in shared memory across the CTA's tiles of an image
-          const int col = et % CW, r0 = (et / CW) * CW;
-          const uint32_t cbyte = p.out_bf16 ? (uint32_t)((col & 7) * 2) : (uint32_t)((col & 3) * 4);
-          const int cchunk = p.out_bf16 ? (col >> 3) : (col >> 2);
-          float s = 0.f, qq = 0.f;
+          // thread -> column (ct % CW), rows [(ct / CW) * RPT, +RPT); accumulated in shared memory across the CTA's tiles of an image
+          const int col = ct % CW, r0 = (ct / CW) * RPT;
+          const uint32_t cbyte = OB ? (uint32_t)((col & 7) * 2) : (uint32_t)((col & 3) * 4);
+          const int cchunk = OB ? (col >> 3) : (col >> 2);
+          float sacc = 0.f, qq = 0.f;
 #pragma unroll 8
-          for (int rr = r0; rr < r0 + CW; ++rr) {
+          for (int rr = r0; rr < r0 + RPT; ++rr) {
             float x;
-            if (p.out_bf16) {
+            if (OB) {
               unsigned short h;
               asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(obuf + swz(rr, cchunk) + cbyte));
               x = __uint_as_float(((uint32_t)h) << 16);
             } else {
               asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(obuf + swz(rr, cchunk) + cbyte));
             }
-            s += x;
+            sacc += x;
             qq = fmaf(x, x, qq);
           }
-          atomicAdd(&st_acc[eg][0][c * CW + col], s);
-          atomicAdd(&st_acc[eg][1][c * CW + col], qq);
+          // the row runs of a column are added in a fixed order by one thread: repeated runs give identical statistics
+          st_part[0][ct] = sacc;
+          st_part[1][ct] = qq;
+          cons_bar();
+          if (ct < CW) {
+            float s2 = 0.f, q2 = 0.f;
+#pragma unroll
+            for (int g = 0; g < 256 / CW; ++g) {
+              s2 += st_part[0][g * CW + ct];
+              q2 += st_part[1][g * CW + ct];
+            }
+            st_acc[0][c * CW + ct] += s2;
+            st_acc[1][c * CW + ct] += q2;
+          }
         }
       }
-      asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-      epi_bar(eg);
-      if (elected) mb_arrive(s_u32(&bar_acc_empty[ab]));
       if (p.ch_stats) {
-        bool flush = tile + 2 >= tile_end;     // this group's next tile is tile + 2
+        bool flush = tile + 1 >= tile_end;
         if (!flush) {
-          const int nt2 = (tile + 2) / p.tiles_m;
-          const int b2 = ((tile + 2) - nt2 * p.tiles_m) / tiles_img;
+          const int nt2 = (tile + 1) / p.tiles_m;
+          const int b2 = ((tile + 1) - nt2 * p.tiles_m) / tiles_img;
           flush = nt2 != nt || b2 != b0;
         }
-        if (flush) {   // (the epi_bar above ordered every thread's shared-memory atomics before these reads)
-          for (int j = et; j < BN; j += 128) {
+        if (flush) {
+          cons_bar();   // every thread's shared-memory atomics are done before these reads
+          for (int j = ct; j < BN; j += 256) {
             float* dst = p.ch_stats + ((long long)b0 * p.Cout + n0 + j) * 2;
-            atomicAdd(dst, st_acc[eg][0][j]);
-            atomicAdd(dst + 1, st_acc[eg][1][j]);
-            st_acc[eg][0][j] = 0.f;
-            st_acc[eg][1][j] = 0.f;
+            atomicAdd(dst, st_acc[0][j]);
+            atomicAdd(dst + 1, st_acc[1][j]);
+            st_acc[0][j] = 0.f;
+            st_acc[1][j] = 0.f;
           }
-          epi_bar(eg);
+          cons_bar();
         }
       }
     }
     if (elected) asm volatile("cp.async.bulk.wait_group 0;" ::: "memory");
-    if (p.dbg && et == 0 && eg == 0) { atomicAdd(p.dbg + 7, w_e); atomicAdd(p.dbg + 8, (unsigned long long)(clock64() - te_begin)); }
-  }
-
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == T3_W_MMA) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(TMEM_COLS) : "memory");
   }
 }
 
@@ -749,16 +587,16 @@ static EncodeTiledFn3 encode_fn3() {
   return fn;
 }
 
-template <int BN, bool X3, bool MG = true, bool DU = false>
+template <int BN, bool X3, bool OB>
 static cudaError_t launch_tc3(const CUtensorMap& b, const CUtensorMap& b2, const CUtensorMap& o, const CUtensorMap& r,
                               const CUtensorMap* sk, const ConvTc3Args& args, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc3_kernel<BN, X3, MG, DU>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc3_kernel<BN, X3, OB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  conv_tc3_kernel<BN, X3, MG, DU><<<grid, T3_THREADS, smem, s>>>(b, b2, o, r, sk[0], sk[1], sk[2], sk[3], args);
+  conv_tc3_kernel<BN, X3, OB><<<grid, T3_THREADS, smem, s>>>(b, b2, o, r, sk[0], sk[1], sk[2], sk[3], args);
   return cudaPeekAtLastError();
 }
 
@@ -767,11 +605,10 @@ static cudaError_t launch_tc3(const CUtensorMap& b, const CUtensorMap& b2, const
 using namespace pdae;
 
 struct pdae_conv_tc3_plan {
-  unsigned long long* dbg = nullptr;
   CUtensorMap tmB, tmB2, tmO, tmR;
   CUtensorMap tmS[4];   // raw halo sources: conv input (C1 | C2), skip-conv input (S1 | S2)
   ConvTc3Args args;
-  int BN, x3, grid, mrg, dual;
+  int BN, x3, grid;
   size_t smem;
 };
 
@@ -817,33 +654,16 @@ extern "C" int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan_out, const void* s
   a.tiles_x = W / T3_TW; a.tiles_y = H / T3_TH; a.tiles_m = a.tiles_x * a.tiles_y * B;
   a.kblocks = Cin / T3_BK; a.kblocks2 = Cs / T3_BK;
   a.has_res = residual != nullptr; a.out_bf16 = out_dtype == PDAE_BF16; a.silu = silu;
-  a.dbg = nullptr;
-  a.dbg_mode = getenv("PDAE_TC3_DBG_MODE") ? atoi(getenv("PDAE_TC3_DBG_MODE")) : 0;
-  if (const char* e = getenv("PDAE_TC3_DBG")) {
-    if (e[0] == '1' && cudaMalloc(&pl->dbg, 16 * sizeof(unsigned long long)) == cudaSuccess) a.dbg = pl->dbg;
-  }
   pl->x3 = x3 ? 1 : 0;
   int BN;
-  const int bn_max = x3 ? 128 : 256;   // split mode: two halo tiles per stage leave room for 128-wide weight tiles only
-  if ((bn_override == 64 || bn_override == 128 || bn_override == 256) && bn_override <= bn_max && Cout % bn_override == 0) BN = bn_override;
-  else if (!x3 && Cout % 256 == 0 && (long long)a.tiles_m * (Cout / 256) >= g_num_sms3) BN = 256;
+  // BN <= 128: each consumer thread holds BN / 2 fp32 accumulators within a 128-register budget
+  if ((bn_override == 64 || bn_override == 128) && Cout % bn_override == 0) BN = bn_override;
   else BN = (Cout % 128 == 0) ? 128 : 64;
   pl->BN = BN;
   a.tiles_total = a.tiles_m * (Cout / BN);
   pl->grid = a.tiles_total < g_num_sms3 ? a.tiles_total : g_num_sms3;
-  const char* em = getenv("PDAE_TC3_MRG128");
-  const bool mrg = x3 && (BN == 64 || !(em && atoi(em) == 0));   // merged [W_hi | W_lo] weight tiles (see the kernel)
-  pl->mrg = mrg ? 1 : 0;
-  {   // EXPERIMENTAL, off by default (PDAE_TC3_DUAL=1 to enable): two MMA issuers (see the kernel) for the 64-wide split-mode
-      // layers.  +8 % on multi-k-block layers and bit-identical results in every single-GPU run, but under torchrun with two
-      // ranks the launch died with 'unspecified launch failure' in 2 of 4 rank-runs (scripts/n2_check.sh; with the second
-      // issuer off the same runs pass) -- an unresolved protocol race, so the product path keeps one issuer.  (In the bf16
-      // mode the heavier epilogue costs more than the second issuer gains: 176 -> 220 us at 64 -> 64.)
-    const char* ed = getenv("PDAE_TC3_DUAL");
-    pl->dual = (x3 && BN == 64 && ed && atoi(ed) == 1) ? 1 : 0;
-  }
-  const int a_stage = (x3 ? 2 : 1) * T3_HALO_BYTES, b_bytes = (mrg ? 2 * BN : BN) * T3_BK * 2;
-  const int staging = ((a.has_res && !x3) ? 4 : 2) * T3_STG_BYTES;   // split mode reads its residual from global memory
+  const int a_stage = (x3 ? 2 : 1) * T3_HALO_BYTES, b_bytes = (x3 ? 2 * BN : BN) * T3_BK * 2;
+  const int staging = ((a.has_res && !x3) ? 2 : 1) * T3_STG_BYTES;   // split mode reads its residual from global memory
   const int budget = 220 * 1024 - 1024 - staging;
   // the transform is software-pipelined, so two halo stages suffice; the weight tiles need depth (bytes in flight from L2)
   int sa = 2;
@@ -851,16 +671,15 @@ extern "C" int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan_out, const void* s
   if (sb > T3_MAX_SB) sb = T3_MAX_SB;
   if (budget - sa * a_stage - sb * b_bytes >= a_stage) sa = 3;
   if (!x3 && a.kblocks2 > 0) {
-    // fused 1x1 skip conv in the fast mode: its k-blocks carry one tap (4 MMAs) per 23 KB raw box, so their cost is the TMA
+    // fused 1x1 skip conv in the fast mode: its k-blocks carry one tap per 23 KB raw box, so their cost is the TMA
     // latency / number of stages in flight -- trade weight-pipeline depth for a fourth halo stage
     int sbw = (budget - 4 * a_stage) / b_bytes;
     if (sbw > T3_MAX_SB) sbw = T3_MAX_SB;
     if (sbw >= 4) { sa = 4; sb = sbw; }
   }
   if (x3 && BN == 64) {
-    // 64-wide split mode: a k-block is short on the tensor pipe (72 narrow MMAs, 8 for a skip block) against the round trip of
-    // its halo stage (raw TMA -> in-place split -> MMAs -> release), so the stage count bounds the rate: three halo stages and
-    // three weight stages beat two and five (skip layers 413 -> 305 us, 3-k-block layers 648 -> 619 us; scripts/ab_dual.sh)
+    // 64-wide split mode: a k-block is short on the tensor pipe against the round trip of its halo stage (raw TMA -> in-place
+    // split -> MMAs -> release), so the stage count bounds the rate: prefer three halo stages
     int sbw = (budget - 3 * a_stage) / b_bytes;
     if (sbw > T3_MAX_SB) sbw = T3_MAX_SB;
     if (sbw >= 3) { sa = 3; sb = sbw; }
@@ -911,7 +730,7 @@ extern "C" int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan_out, const void* s
   {
     cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout, (cuuint64_t)(9 * nmat)};
     cuuint64_t strides[2] = {(cuuint64_t)Cin * 2, (cuuint64_t)Cout * Cin * 2};
-    cuuint32_t box[3] = {(cuuint32_t)T3_BK, (cuuint32_t)BN, (cuuint32_t)(mrg ? 2 : 1)};
+    cuuint32_t box[3] = {(cuuint32_t)T3_BK, (cuuint32_t)BN, (cuuint32_t)nmat};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&pl->tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(w), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -922,7 +741,7 @@ extern "C" int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan_out, const void* s
   if (Cs > 0) {
     cuuint64_t dims[3] = {(cuuint64_t)Cs, (cuuint64_t)Cout, (cuuint64_t)nmat};
     cuuint64_t strides[2] = {(cuuint64_t)Cs * 2, (cuuint64_t)Cout * Cs * 2};
-    cuuint32_t box[3] = {(cuuint32_t)T3_BK, (cuuint32_t)BN, (cuuint32_t)(mrg ? 2 : 1)};
+    cuuint32_t box[3] = {(cuuint32_t)T3_BK, (cuuint32_t)BN, (cuuint32_t)nmat};
     cuuint32_t estr[3] = {1, 1, 1};
     CUresult r = enc(&pl->tmB2, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(w_skip), dims, strides, box, estr,
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
@@ -954,39 +773,17 @@ extern "C" int pdae_conv_tc3_run(const pdae_conv_tc3_plan* pl, pdae_stream_t str
   PDAE_REQUIRE(pl, "conv_tc3_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
-#define T3_GO(...) launch_tc3<__VA_ARGS__>(pl->tmB, pl->tmB2, pl->tmO, pl->tmR, pl->tmS, pl->args, pl->grid, pl->smem, s)
-  if (pl->x3) {
-    if (pl->BN == 64) e = pl->dual ? T3_GO(64, true, true, true) : T3_GO(64, true, true, false);
-    else if (pl->mrg) e = T3_GO(128, true, true, false);
-    else e = T3_GO(128, true, false, false);
-  } else {
-    switch (pl->BN) {
-      case 64: e = T3_GO(64, false, true, false); break;
-      case 128: e = T3_GO(128, false, true, false); break;
-      default: e = T3_GO(256, false, true, false); break;
-    }
-  }
+#define T3_GO(BN, X3) (pl->args.out_bf16 ? launch_tc3<BN, X3, true>(pl->tmB, pl->tmB2, pl->tmO, pl->tmR, pl->tmS, pl->args, pl->grid, pl->smem, s) \
+                                         : launch_tc3<BN, X3, false>(pl->tmB, pl->tmB2, pl->tmO, pl->tmR, pl->tmS, pl->args, pl->grid, pl->smem, s))
+  if (pl->x3) e = pl->BN == 64 ? T3_GO(64, true) : T3_GO(128, true);
+  else e = pl->BN == 64 ? T3_GO(64, false) : T3_GO(128, false);
 #undef T3_GO
   if (e != cudaSuccess) {
     (void)cudaGetLastError();
     set_error("launch of conv_tc3_kernel<%d,%d> failed: %s", pl->BN, pl->x3, cudaGetErrorString(e));
     return PDAE_ECUDA;
   }
-  if (pl->dbg) {   // tuning aid only: synchronous read-out of the per-role wait counters (sums over all CTAs)
-    unsigned long long h[16];
-    cudaStreamSynchronize(s);
-    cudaMemcpy(h, pl->dbg, sizeof(h), cudaMemcpyDeviceToHost);
-    cudaMemset(pl->dbg, 0, sizeof(h));
-    const double n = (double)pl->grid;
-    fprintf(stderr, "[tc3 dbg] BN=%d x3=%d grid=%d sa=%d sb=%d | per CTA kcycles: mma wait a_full %.0f b_full %.0f acc_empty %.0f | rawprod wait a_empty "
-            "%.0f | bprod wait b_empty %.0f | xform wait raw %.0f of %.0f | epi(g0) wait acc_full %.0f of %.0f\n", pl->BN, pl->x3, pl->grid,
-            pl->args.sa, pl->args.sb, h[0] / n / 1e3, h[1] / n / 1e3, h[2] / n / 1e3, h[3] / n / 1e3, h[4] / n / 1e3, h[5] / n / 1e3, h[6] / n / 1e3,
-            h[7] / n / 1e3, h[8] / n / 1e3);
-  }
   return PDAE_OK;
 }
 
-extern "C" void pdae_conv_tc3_destroy(pdae_conv_tc3_plan* pl) {
-  if (pl && pl->dbg) cudaFree(pl->dbg);
-  delete pl;
-}
+extern "C" void pdae_conv_tc3_destroy(pdae_conv_tc3_plan* pl) { delete pl; }

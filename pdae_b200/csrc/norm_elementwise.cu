@@ -677,8 +677,8 @@ extern "C" int pdae_device_check(void) {
     set_error("no CUDA device available");
     return PDAE_ENODEV;
   }
-  if (prop.major != 10) {
-    set_error("device is sm_%d%d; pdae_b200 is built for sm_100a only", prop.major, prop.minor);
+  if (prop.major != 9 || prop.minor != 0) {
+    set_error("device is sm_%d%d; pdae_b200 is built for sm_90a only", prop.major, prop.minor);
     return PDAE_ENODEV;
   }
   return PDAE_OK;

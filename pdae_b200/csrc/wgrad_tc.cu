@@ -1,34 +1,37 @@
-// wgrad_tc -- weight gradient of a stride-1 3x3 / 1x1 "same" convolution on the tensor cores (sm_100a), fp32-grade.
+// wgrad_tc -- weight gradient of a stride-1 3x3 / 1x1 "same" convolution on the tensor cores (sm_90a), fp32-grade.
 //
 //   dW[tap][cin][cout] = sum over (b, y, x) of  act[b, y+dy, x+dx, cin] * dY[b, y, x, cout]        (autograd of F.conv2d,
 //   model/module.py:241-243, 255-259 under trainer/train_representation_learning.py:112 loss.backward())
 //
-// As a GEMM the contraction runs over PIXELS while both operands are NHWC (channels contiguous): both are MN-major UMMA
+// As a GEMM the contraction runs over PIXELS while both operands are NHWC (channels contiguous): both are MN-major wgmma
 // operands.  A TMA box [64 pixels][64 channels] with SWIZZLE_128B is exactly the canonical MN-major SW128 atom stack
 // (8 pixel rows x 128 B per atom, stride-byte-offset 1024 B between 8-row groups); a second box one leading-byte-offset
-// further supplies channels 64-127.  One MMA = 128 (M channels) x BN (N channels) x 16 pixels.
+// further supplies channels 64-127.  One k-step = 128 (M channels) x BN (N channels) x 16 pixels, as two m64 wgmmas (one per
+// consumer warpgroup).
 //
 // Operands arrive split, [hi | lo | hi] channel blocks (a = hi + lo, bf16 each): every product is
-// a_hi*d_hi + a_lo*d_hi + a_hi*d_lo accumulated in fp32 in TMEM -- the same fp32-grade scheme as the forward / dgrad convs.
+// a_hi*d_hi + a_lo*d_hi + a_hi*d_lo accumulated in fp32 registers -- the same fp32-grade scheme as the forward / dgrad convs.
 //
 // Work item = (tap, M chunk of 128 channels, N chunk of BN channels, 64-pixel tile).  Items are dealt to the persistent CTAs
-// in contiguous ranges (split-K over pixels); a CTA accumulates in TMEM while consecutive items belong to the same
+// in contiguous ranges (split-K over pixels); a CTA accumulates in registers while consecutive items belong to the same
 // (tap, M chunk, N chunk) and then adds its partial sums to dW with fp32 reductions.
-//   warp 4: TMA producer, warp 5: MMA issuer (warp-uniform loops, elect.sync), warps 0-3: epilogue (one TMEM lane quadrant each).
+//   warp 8: TMA producer (warp-uniform loop, elect.sync), warps 0-7: two consumer warpgroups, warpgroup g owning accumulator
+//   rows [64 g, 64 g + 64) (wgmma, then the reductions straight from the accumulator fragments).
 // The tap shift is applied to whichever operand is the activation (4-D box at shifted coordinates, out-of-image = zero = padding).
-// `a_is_act` selects which tensor sits on the M side: with dY there (M = cout) the 32 lanes of a warp reduce into 32
-// consecutive dW addresses (coalesced), which is the preferred form whenever Cout % 128 == 0.  When neither channel count is a
+// `a_is_act` selects which tensor sits on the M side: with dY there (M = cout), which is the preferred form whenever
+// Cout % 128 == 0.  When neither channel count is a
 // multiple of 128 (64 -> 64, 192 -> 64) the M side is the activation in 64-channel chunks and the two 64-row halves of the
 // accumulator hold two different TAPS of it ("pair" mode; the odd ninth tap is paired with a discarded duplicate).
 #include <cuda.h>
 
 #include "common.cuh"
+#include "wgmma.cuh"
 
 namespace pdae {
 
 constexpr int WG_KT = 64;                 // pixels per k-tile (= rows of one TMA box)
 constexpr int WG_BOX = WG_KT * 128;       // bytes of one [64 px][64 ch] box
-constexpr int WG_THREADS = 192;
+constexpr int WG_THREADS = 288;
 constexpr int WG_MAX_ST = 4;
 
 struct WgradArgs {
@@ -77,37 +80,10 @@ __device__ __forceinline__ void tma_ld4(uint32_t dst, const CUtensorMap* m, uint
       ::"r"(dst), "l"(m), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
-// MN-major SWIZZLE_128B operand: 64-element (128 B) channel blocks `lbo` bytes apart, 8-pixel row groups 1024 B apart
-__device__ __forceinline__ uint64_t mn_desc(uint32_t saddr, uint32_t lbo) {
-  return (uint64_t)((saddr & 0x3FFFFu) >> 4) | ((uint64_t)(lbo >> 4) << 16) | ((uint64_t)(1024u >> 4) << 32) | (1ull << 46) |
-         (2ull << 61);
-}
-__device__ __forceinline__ void umma(uint32_t tmem_d, uint64_t a, uint64_t b, uint32_t idesc, uint32_t accum) {
-  asm volatile(
-      "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}"
-      ::"r"(tmem_d), "l"(a), "l"(b), "r"(idesc), "r"(accum)
-      : "memory");
-}
-__device__ __forceinline__ void umma_commit_to(uint32_t bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(bar) : "memory");
-}
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
   return pred != 0;
-}
-__device__ __forceinline__ void tmem_ld32(uint32_t taddr, uint32_t* v) {
-  asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0,%1,%2,%3,%4,%5,%6,%7,%8,%9,%10,%11,%12,%13,%14,%15,%16,%17,%18,%19,%20,%21,%22,%23,%24,%25,%26,%27,%28,%29,%30,%31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]), "=r"(v[8]),
-        "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]), "=r"(v[16]),
-        "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]), "=r"(v[24]),
-        "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
-      : "memory");
 }
 }  // namespace wg
 
@@ -116,8 +92,7 @@ __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, WgradArgs p) {
   using namespace wg;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_full[WG_MAX_ST], bar_empty[WG_MAX_ST], bar_acc_full, bar_acc_empty;
-  __shared__ uint32_t tmem_slot;
+  __shared__ __align__(8) uint64_t bar_full[WG_MAX_ST], bar_empty[WG_MAX_ST];
   constexpr int NBOX_B = BN / 64;                       // 64-channel boxes of the N-side tile
   constexpr int A_BYTES = 2 * WG_BOX;                   // M = 128 channels = two boxes
   constexpr int B_BYTES = NBOX_B * WG_BOX;
@@ -132,27 +107,16 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
       mb_init(s_u32(&bar_full[s]), 1);
-      mb_init(s_u32(&bar_empty[s]), 1);
+      mb_init(s_u32(&bar_empty[s]), 8);   // one arrive per consumer warp
     }
-    mb_init(s_u32(&bar_acc_full), 1);
-    mb_init(s_u32(&bar_acc_empty), 1);
     asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
     asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmA) : "memory");
     asm volatile("prefetch.tensormap [%0];" ::"l"(&tmB) : "memory");
   }
-  if (warp == 5) {
-    __syncwarp();
-    asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(s_u32(&tmem_slot)), "n"(BN < 32 ? 32 : BN)
-                 : "memory");
-    asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
   __syncthreads();
-  asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-  const uint32_t tmem_base = tmem_slot;
 
-  if (warp == 4) {
+  if (warp == 8) {
     // ================= TMA producer =================
     int s = 0;
     uint32_t ph = 0;
@@ -198,98 +162,57 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       __syncwarp();
       if (++s == S) { s = 0; ph ^= 1u; }
     }
-  } else if (warp == 5) {
-    // ================= MMA issuer =================
-    constexpr uint32_t IDESC = (1u << 4) | (1u << 7) | (1u << 10) | (1u << 15) | (1u << 16) | ((uint32_t)(BN >> 3) << 17) |
-                               ((uint32_t)(128 >> 4) << 24);   // fp32 accumulate, bf16 x bf16, A and B MN-major
-    const uint32_t tmem_d = __shfl_sync(0xffffffffu, tmem_base, 0);
-    int s = 0, ngroups = 0;
+  } else {
+    // ================= consumers: warpgroup wg = M box wg (accumulator rows [64 wg, 64 wg + 64)) =================
+    const int wgi = warp >> 2, t = threadIdx.x & 127;
+    float acc[BN / 2];
+#pragma unroll
+    for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
+    // fp32 reductions of a finished (tap, M chunk, N chunk) group into dW, straight from the accumulator fragments
+    auto flush = [&](long long gid) {
+      int gg = (int)gid;
+      const int nc = gg % p.nchunks; gg /= p.nchunks;
+      const int mc = gg % p.mchunks;
+      const int tap = gg / p.mchunks;
+      const int tap_w = p.pair ? 2 * tap + wgi : tap;             // pair mode: rows 64-127 belong to the second tap
+      if (tap_w >= p.taps) return;
+      float* base = p.dw + (long long)tap_w * p.stap + (long long)(nc * BN) * p.sn;
+#pragma unroll
+      for (int i = 0; i < BN / 2; ++i) {
+        const int m = wgmma::frag_row(t, i);
+        const int ch_m = p.pair ? mc * 64 + m : mc * 128 + 64 * wgi + m;
+        atomicAdd(base + (long long)ch_m * p.sm + (long long)wgmma::frag_col(t, i) * p.sn, acc[i]);
+      }
+    };
+    int s = 0;
     uint32_t ph = 0;
     long long cur_g = -1;
     for (long long it = it_begin; it < it_end; ++it) {
       const long long g = it / p.ktiles;
       const bool first = g != cur_g;
       if (first) {
-        if (cur_g >= 0) {                      // previous group complete: hand the accumulator to the epilogue ...
-          if (elect_one()) umma_commit_to(s_u32(&bar_acc_full));
-          __syncwarp();
-        }
-        if (ngroups > 0) {                     // ... and wait until it has been drained
-          mb_wait(s_u32(&bar_acc_empty), (uint32_t)((ngroups - 1) & 1));
-          asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        }
+        if (cur_g >= 0) flush(cur_g);
         cur_g = g;
-        ++ngroups;
       }
       mb_wait(s_u32(&bar_full[s]), ph);
-      asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-      const uint32_t base = smem0 + (uint32_t)(s * STAGE);
-      const uint64_t a_hi = mn_desc(base, WG_BOX), a_lo = mn_desc(base + A_BYTES, WG_BOX);
-      const uint64_t b_hi = mn_desc(base + 2 * A_BYTES, WG_BOX), b_lo = mn_desc(base + 2 * A_BYTES + B_BYTES, WG_BOX);
-      const uint32_t bar_e = s_u32(&bar_empty[s]);
-      if (elect_one()) {
+      const uint32_t base = smem0 + (uint32_t)(s * STAGE) + (uint32_t)(wgi * WG_BOX);
+      const uint64_t a_hi = wgmma::desc_sw128(base, WG_BOX, 1024u), a_lo = wgmma::desc_sw128(base + A_BYTES, WG_BOX, 1024u);
+      const uint32_t bb = smem0 + (uint32_t)(s * STAGE) + 2u * A_BYTES;
+      const uint64_t b_hi = wgmma::desc_sw128(bb, WG_BOX, 1024u), b_lo = wgmma::desc_sw128(bb + B_BYTES, WG_BOX, 1024u);
+      wgmma::fence();
 #pragma unroll
-        for (int k = 0; k < WG_KT / 16; ++k) {           // 16 pixels per MMA = 16 rows x 128 B = 2048 B = 128 descriptor units
-          const uint64_t o = (uint64_t)(k * 128);
-          umma(tmem_d, a_hi + o, b_hi + o, IDESC, (uint32_t)(!(first && k == 0)));
-          umma(tmem_d, a_lo + o, b_hi + o, IDESC, 1u);
-          umma(tmem_d, a_hi + o, b_lo + o, IDESC, 1u);
-        }
-        umma_commit_to(bar_e);
+      for (int k = 0; k < WG_KT / 16; ++k) {           // 16 pixels per k-step = 16 rows x 128 B = 2048 B = 128 descriptor units
+        const uint64_t o = (uint64_t)(k * 128);
+        wgmma::mma<BN, 1>(acc, a_hi + o, b_hi + o, (uint32_t)(!(first && k == 0)));
+        wgmma::mma<BN, 1>(acc, a_lo + o, b_hi + o, 1u);
+        wgmma::mma<BN, 1>(acc, a_hi + o, b_lo + o, 1u);
       }
-      __syncwarp();
+      wgmma::commit();
+      wgmma::wait<0>();
+      if (lane == 0) mb_arrive(s_u32(&bar_empty[s]));
       if (++s == S) { s = 0; ph ^= 1u; }
     }
-    if (cur_g >= 0) {
-      if (elect_one()) umma_commit_to(s_u32(&bar_acc_full));
-      __syncwarp();
-    }
-  } else {
-    // ================= epilogue: TMEM -> fp32 reductions into dW =================
-    const int q = warp & 3;
-    const int m = q * 32 + lane;               // accumulator row = channel on the M side
-    const int et = threadIdx.x;                // 0..127
-    int ngroups = 0;
-    long long cur_g = -1;
-    for (long long it = it_begin; it <= it_end; ++it) {
-      const long long g = it < it_end ? it / p.ktiles : -2;
-      if (g == cur_g) continue;
-      if (cur_g >= 0) {
-        mb_wait(s_u32(&bar_acc_full), (uint32_t)((ngroups - 1) & 1));
-        asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory");
-        int gg = (int)cur_g;
-        const int nc = gg % p.nchunks; gg /= p.nchunks;
-        const int mc = gg % p.mchunks;
-        const int tap = gg / p.mchunks;
-        const int tap_w = p.pair ? 2 * tap + (m >> 6) : tap;             // pair mode: rows 64-127 belong to the second tap
-        const int ch_m = p.pair ? mc * 64 + (m & 63) : mc * 128 + m;
-        const bool live = tap_w < p.taps;
-        float* dst = p.dw + (long long)tap_w * p.stap + (long long)ch_m * p.sm + (long long)(nc * BN) * p.sn;
-        const uint32_t tacc = tmem_base + ((uint32_t)(q * 32) << 16);
-#pragma unroll 1
-        for (int c = 0; c < BN / 32; ++c) {
-          uint32_t v[32];
-          tmem_ld32(tacc + (uint32_t)(c * 32), v);
-          asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory");
-#pragma unroll
-          if (live) {
-#pragma unroll
-            for (int j = 0; j < 32; ++j) atomicAdd(dst + (long long)(c * 32 + j) * p.sn, __uint_as_float(v[j]));
-          }
-        }
-        asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-        asm volatile("bar.sync 1, 128;" ::: "memory");
-        if (et == 0) mb_arrive(s_u32(&bar_acc_empty));
-      }
-      cur_g = g;
-      if (g >= 0) ++ngroups;
-    }
-  }
-  asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory");
-  __syncthreads();
-  if (warp == 5) {
-    __syncwarp();
-    asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(tmem_base), "n"(BN < 32 ? 32 : BN) : "memory");
+    if (cur_g >= 0) flush(cur_g);
   }
 }
 

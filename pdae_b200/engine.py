@@ -8,7 +8,7 @@ PyTorch is used here only for device memory and streams.
 Precision modes
   * ``fp32``: every contraction on CUDA cores in fp32 (pdae_conv2d_simt / pdae_attention_simt).  This is
     the mode that holds rtol 1e-3 / atol 1e-4 against the CPU oracle.
-  * ``bf16``: convolutions whose shape allows it run on the tcgen05 tensor-core kernel with bf16 operands
+  * ``bf16``: convolutions whose shape allows it run on the wgmma tensor-core kernel with bf16 operands
     and fp32 accumulation (pdae_conv_tc_*); the residual stream, GroupNorm statistics, embeddings and
     the DDIM update stay fp32.
 """
@@ -28,8 +28,8 @@ _STREAM = object()  # placeholder replaced by the current stream at run time
 
 _default_precision = "bf16"
 # "fp32"   : CUDA-core fp32 arithmetic everywhere (parity / training mode)
-# "bf16"   : tcgen05 bf16 MMAs, bf16 activations and residual stream (the fast mode; stated tolerance rel-L2 <= 2e-2)
-# "bf16x3" : tcgen05 bf16 MMAs on split operands (a = hi + lo, three products per term), fp32 residual stream and GroupNorm
+# "bf16"   : wgmma bf16 MMAs, bf16 activations and residual stream (the fast mode; stated tolerance rel-L2 <= 2e-2)
+# "bf16x3" : wgmma bf16 MMAs on split operands (a = hi + lo, three products per term), fp32 residual stream and GroupNorm
 #            inputs: fp32-grade results (meets the fp32 tolerance) at ~3x the MMA work of "bf16"
 PRECISIONS = ("fp32", "bf16", "bf16x3")
 
@@ -138,7 +138,7 @@ class Plan:
         # conv_tc3: GroupNorm-apply / AdaGN / SiLU (and the bf16x3 hi/lo split) fused into the conv's operand path -- the
         # activated tensor never exists in HBM.  PDAE_TC3=0 restores the separate gn_apply + conv_tc2 pair (A/B aid).
         self.fuse_prologue = self.tc and self.v2 and os.environ.get("PDAE_TC3", "1") == "1"
-        self.fuse_coef = os.environ.get("PDAE_FUSE_COEF", "0") == "1"   # GN coefficients inside gn_apply: measured 0.15 ms/step SLOWER under graph replay (profiles/README.md) -> off
+        self.fuse_coef = os.environ.get("PDAE_FUSE_COEF", "0") == "1"   # GN coefficients inside gn_apply (A/B aid, off by default)
         self.L = _native.lib()
         self.ops: List[Tuple[str, list]] = []
         # ops recorded inside `with P.prologue():` depend only on inputs that are constant over a sampling loop (z):
@@ -428,7 +428,7 @@ class Plan:
 
     def gemm_tc(self, a, a_ld, a_bs, b, b_ld, b_bs, out, out_ld, out_bs, *, batch, M, N, K, out_dtype,
                 softmax_alpha: Optional[float] = None, flops: Optional[float] = None) -> None:
-        """Batched out_i = A_i (MxK) * B_i (NxK)^T on the persistent tcgen05 kernel; a/b/out are Buf or BufView.
+        """Batched out_i = A_i (MxK) * B_i (NxK)^T on the persistent wgmma kernel; a/b/out are Buf or BufView.
         softmax_alpha: store softmax_rows(alpha * out_i) (bf16) instead -- needs N in {64,128,256} (row inside one tile)."""
         if softmax_alpha is not None:
             assert out_dtype == torch.bfloat16 and N in (64, 128, 256)
@@ -614,7 +614,7 @@ class Plan:
                 return None
             stats = self.new_stats(B, Cout) if want_stats else None
             if skip is not None:
-                # fused 1x1 skip conv (model/module.py:268-276): extra K blocks accumulated into the same TMEM tile
+                # fused 1x1 skip conv (model/module.py:268-276): extra K blocks accumulated into the same accumulator tile
                 sk_in, sw, sb, Cin2 = skip   # sk_in: a bf16 buffer, or (buf_a, Ca, buf_b, Cb) = their channel concat
                 assert residual is None
                 if isinstance(sk_in, tuple):

@@ -169,7 +169,7 @@ class PlannedModule(nn.Module):
         p = next(self.parameters())
         if not p.is_cuda:
             raise _native.NativeError(f"{type(self).__name__}: parameters are on {p.device}; pdae_b200 runs on CUDA "
-                                      "(sm_100) only -- there is no CPU fallback")
+                                      "(sm_90) only -- there is no CPU fallback")
         return p.device
 
     def __deepcopy__(self, memo):
@@ -470,7 +470,7 @@ class AttentionBlock(PlannedModule):
                            act_dtype=torch.bfloat16 if tcq else torch.float32)
         heads, ch = self.num_heads, C // self.num_heads
         if tcq and P.can_gemm_tc(T, T, ch) and P.can_gemm_tc(T, ch, T):
-            # ---- tensor-core attention: bf16 qkv -> S = Q K^T (batched tcgen05 GEMM) -> softmax -> P V ----
+            # ---- tensor-core attention: bf16 qkv -> S = Q K^T (batched wgmma GEMM) -> softmax -> P V ----
             qkv = P.new((B, T, 3 * C), torch.bfloat16, "qkv")
             P.conv(xn, self.qkv.weight, self.qkv.bias, qkv, B=B, H=H, W=W, Cin=C, Cout=3 * C, k=1)
             vT = P.new((B * heads, ch, T), torch.bfloat16, "vT")
@@ -483,7 +483,7 @@ class AttentionBlock(PlannedModule):
             fuse_sm = T in (64, 128, 256) and os.environ.get("PDAE_FUSE_SOFTMAX", "1") == "1"
             S = None if fuse_sm else P.new((B * heads, T, T), torch.float32, "att_scores")
             for h in range(heads):
-                if fuse_sm:   # a whole score row sits in one TMEM accumulator tile: softmax in the GEMM epilogue
+                if fuse_sm:   # a whole score row sits in one accumulator tile: softmax in the GEMM epilogue
                     P.gemm_tc(qkv.at(h * hs_), 3 * C, T * 3 * C, qkv.at(h * hs_ + ko), 3 * C, T * 3 * C,
                               Pm.at(h * T * T), T, heads * T * T, batch=B, M=T, N=T, K=ch, out_dtype=torch.bfloat16,
                               softmax_alpha=alpha)
@@ -497,7 +497,7 @@ class AttentionBlock(PlannedModule):
                           att.at(h * ch), C, T * C, batch=B, M=T, N=ch, K=T, out_dtype=torch.bfloat16)
         elif tcq and tape is None and P.can_gemm_x3(T, T, ch) and P.can_gemm_x3(T, ch, T):
             # ---- split-operand tensor-core attention (fp32-grade): fp32 qkv -> [hi|lo|hi] x [hi|hi|lo] operand blocks ->
-            # S = Q K^T (fp32) -> fp32 softmax, split -> A = P V (fp32); every product is three bf16 tcgen05 MMAs ----
+            # S = Q K^T (fp32) -> fp32 softmax, split -> A = P V (fp32); every product is three bf16 wgmma MMAs ----
             qkv = P.new((B, T, 3 * C), torch.float32, "qkv")
             P.conv(xn, self.qkv.weight, self.qkv.bias, qkv, B=B, H=H, W=W, Cin=C, Cout=3 * C, k=1)
             Z = B * heads

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
-"""Generate tests/golden/*.npz by running the REAL reference (ckczzj/PDAE at /root/reference).
+"""Generate tests/golden/*.npz by running the REAL reference (ckczzj/PDAE, sources at $PDAE_REFERENCE_DIR).
 
-Run only in the build container (the GPU box has no /root/reference):
+Run only where the reference sources are available:
     python tests/golden/make_golden.py
 Each fixture stores the config (JSON), the input seeds and the reference outputs.  Weights are NOT
 stored: both sides regenerate them with pdae_b200.utils.synth (numpy PCG64 keyed by parameter
@@ -18,7 +18,7 @@ import torch
 HERE = os.path.dirname(os.path.abspath(__file__))
 ROOT = os.path.dirname(os.path.dirname(HERE))
 sys.path.insert(0, ROOT)
-sys.path.insert(0, "/root/reference")
+sys.path.insert(0, os.environ["PDAE_REFERENCE_DIR"])
 
 from pdae_b200.utils.synth import fill_module_, synth_images, synth_normal  # noqa: E402
 

@@ -6,7 +6,8 @@ import sys
 
 HERE = os.path.dirname(os.path.abspath(__file__))
 sys.path.insert(0, os.path.dirname(os.path.dirname(HERE)))
-sys.path.insert(0, "/root/reference")
+REF = os.environ["PDAE_REFERENCE_DIR"]
+sys.path.insert(0, REF)
 import yaml  # noqa: E402
 from model.unet import UNet  # noqa: E402
 from model.shift_unet import ShiftUNet  # noqa: E402
@@ -14,7 +15,7 @@ from model.mlp_skip_net import MLPSkipNet  # noqa: E402
 from model.representation_learning.encoder import CELEBA64Encoder, FFHQEncoder  # noqa: E402
 from tests.configs import CELEBA64_PROXY, FFHQ128_PROXY, FFHQ_LATENT  # noqa: E402
 
-mnist = yaml.load(open("/root/reference/config/mnist_regular.yml"), Loader=yaml.FullLoader)["denoise_fn_config"]
+mnist = yaml.load(open(os.path.join(REF, "config", "mnist_regular.yml")), Loader=yaml.FullLoader)["denoise_fn_config"]
 mods = {
     "unet_mnist": (UNet(**mnist), mnist),
     "shiftunet_celeba64_proxy": (ShiftUNet(latent_dim=512, **CELEBA64_PROXY), dict(CELEBA64_PROXY, latent_dim=512)),

@@ -1,4 +1,4 @@
-"""tcgen05/TMA convolution vs the fp32 CUDA-core kernel on identical (bf16-rounded) operands, plus the
+"""wgmma/TMA convolution vs the fp32 CUDA-core kernel on identical (bf16-rounded) operands, plus the
 CUDA-core kernel vs torch's CPU conv2d (the oracle's arithmetic).  Differences between the two GPU kernels can
 only come from accumulation order, so the tolerance is tight."""
 import pytest
@@ -184,7 +184,7 @@ def test_head_conv_smalln():
 
 @pytest.mark.parametrize("T,K,batch", [(256, 128, 3), (128, 64, 5), (256, 512, 2)])
 def test_softmax_gemm_epilogue(T, K, batch):
-    """P = softmax_rows(alpha * Q K^T) with the softmax inside the tcgen05 GEMM epilogue (scores stay in TMEM) vs torch."""
+    """P = softmax_rows(alpha * Q K^T) with the softmax inside the wgmma GEMM epilogue (scores stay in registers) vs torch."""
     from pdae_b200.engine import Plan
     g = torch.Generator(device="cpu").manual_seed(17)
     q = torch.randn(batch, T, K, generator=g).to(torch.bfloat16)

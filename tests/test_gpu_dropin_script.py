@@ -5,7 +5,8 @@ classes) executes on the pdae_b200 kernels after `pdae_b200.dropin.install()`.
 
 Only what the offline box lacks is stubbed -- matplotlib / lmdb / lpips (third-party imports of utils/utils.py and
 metric/lpips, SURVEY D9), a synthetic in-memory dataset registered under the reference's `dataset` module, and a
-synthetic checkpoint + config files.  Needs baseline/_ref (vendored by __graft_entry__.build())."""
+synthetic checkpoint + config files.  Needs oracle/_ref (installed by __graft_entry__.build() from the original project's
+sources, oracle/install_reference.py); skips without it."""
 import json
 import os
 import socket
@@ -17,7 +18,7 @@ import pytest
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-REF = os.path.join(ROOT, "baseline", "_ref")
+REF = os.path.join(ROOT, "oracle", "_ref")
 
 SCRIPT = r'''
 import argparse, json, os, sys, types
@@ -104,7 +105,7 @@ def _free_port():
 
 def test_reference_autoencoding_eval_script_runs_on_native_kernels(tmp_path):
     if not os.path.exists(os.path.join(REF, "sampler", "autoencoding_eval.py")):
-        pytest.skip("baseline/_ref not vendored (run __graft_entry__.build() where /root/reference exists)")
+        pytest.skip("oracle/_ref not installed (__graft_entry__.build() installs it when the original project's sources are available)")
     script = tmp_path / "run_ref_script.py"
     script.write_text(textwrap.dedent(SCRIPT))
     env = dict(os.environ, RANK="0", WORLD_SIZE="1", LOCAL_RANK="0", LOCAL_WORLD_SIZE="1", MASTER_ADDR="127.0.0.1",

@@ -130,7 +130,7 @@ def test_oracle_agrees_on_gpu_inputs_at_larger_shape():
 
 @pytest.mark.parametrize("C,heads,new_order", [(128, 1, False), (128, 2, False), (128, 2, True), (256, 1, True)])
 def test_attention_tensor_core(C, heads, new_order):
-    """16x16 tokens (T=256): the bf16 path runs QK^T and PV as batched tcgen05 GEMMs -- vs the CPU oracle."""
+    """16x16 tokens (T=256): the bf16 path runs QK^T and PV as batched wgmma GEMMs -- vs the CPU oracle."""
     from pdae_b200.model import module as pm
     from pdae_b200.utils.synth import fill_module_, synth_normal
     m = fill_module_(pm.AttentionBlock(C, heads, -1, new_order), seed=31).eval()
@@ -144,7 +144,7 @@ def test_attention_tensor_core(C, heads, new_order):
             y = m(x.cuda())
         check(y, ref, precision, f"attention C={C} heads={heads} new={new_order}")
     plan3 = [v for k, v in m._plans().items() if k[1] == "bf16x3"][0][0]
-    # split-operand mode: QK^T and PV as batched tcgen05 GEMMs on [hi|lo|hi] x [hi|hi|lo] operand blocks (fp32-grade)
+    # split-operand mode: QK^T and PV as batched wgmma GEMMs on [hi|lo|hi] x [hi|hi|lo] operand blocks (fp32-grade)
     assert any(op[0] == "qkv_split3" for op in plan3.ops) and not any(op[0] == "attention_simt" for op in plan3.ops)
     plan = [v for k, v in m._plans().items() if k[1] == "bf16"][0][0]
     if plan.v2:   # (the legacy v1 kernel, PDAE_TC_V1=1, has no batched-GEMM mode: CUDA-core attention there)

@@ -1,4 +1,4 @@
-"""The C-ABI library builds for sm_100a, loads, and exports every symbol include/pdae_b200.h declares (no GPU needed)."""
+"""The C-ABI library builds for sm_90a, loads, and exports every symbol include/pdae_b200.h declares (no GPU needed)."""
 import ctypes
 import os
 import re
@@ -34,8 +34,8 @@ def test_abi_version_and_error_string():
     assert rc == -1 and b"unsupported" in L.pdae_last_error()
 
 
-def test_sass_is_blackwell_native():
-    """tcgen05.mma -> UTCHMMA, TMA -> UTMALDG, tcgen05.ld -> LDTM must be present in the sm_100a cubin."""
+def test_sass_is_hopper_native():
+    """wgmma -> HGMMA, TMA load / store -> UTMALDG / UTMASTG must be present in the sm_90a cubin."""
     import shutil
     import subprocess
     cuobjdump = shutil.which("cuobjdump") or "/usr/local/cuda/bin/cuobjdump"
@@ -43,6 +43,6 @@ def test_sass_is_blackwell_native():
         import pytest
         pytest.skip("cuobjdump not available")
     sass = subprocess.run([cuobjdump, "-sass", _native.LIB_PATH], capture_output=True, text=True).stdout
-    for mnem in ("UTCHMMA", "UTMALDG", "LDTM"):
+    for mnem in ("HGMMA", "UTMALDG", "UTMASTG"):
         assert mnem in sass, mnem
-    assert "sm_100a" in sass
+    assert "sm_90a" in sass

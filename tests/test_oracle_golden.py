@@ -1,6 +1,6 @@
 """Pin the CPU oracle (oracle/pdae_oracle.py) against the fixtures recorded from the REAL reference
-(tests/golden/make_golden.py).  CPU only; this is what makes the oracle trustworthy on the GPU box, where
-/root/reference does not exist."""
+(tests/golden/make_golden.py).  CPU only; this is what makes the oracle trustworthy where the reference sources
+are not available."""
 import numpy as np
 import pytest
 import torch
