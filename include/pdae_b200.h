@@ -86,15 +86,6 @@ int pdae_gn_apply(const void* src1, int src1_dtype, int C1, const void* src2, in
  * a_hi*W_hi + a_lo*W_hi + a_hi*W_lo.  out_raw (optional): fp32 plain [..][C] or bf16 split [..][3C] per raw_dtype.        */
 int pdae_gn_apply_split3(const float* src1, int C1, const float* src2, int C2, const float* ab, int silu, int resample, int B,
                          int H, int W, void* out_act3_bf16, void* out_raw, int raw_dtype, pdae_stream_t stream);
-/* GroupNorm(32) + affine/AdaGN + SiLU in ONE launch (the gn_coef_ch + gn_apply pair): coefficients are derived in each
- * CTA's prologue from the per-channel (sum, sum^2) of the sources ([B][C][2] fp32, as accumulated by the conv epilogue or
- * pdae_ch_stats).  No resampling; out_act is bf16 NHWC [B][H][W][C1+C2]; out_raw (optional) the un-normalised concat in
- * raw_dtype.  Replaces nn.GroupNorm + scale/shift + nn.SiLU of model/module.py:241-243,255-258,291-293,380-381.
- * C1, C2 multiples of 8, 64 <= C1+C2 <= 2048, (C1+C2) % 32 == 0.                                                        */
-int pdae_gn_norm_apply(const void* src1, int src1_dtype, int C1, const float* chs1, const void* src2, int src2_dtype, int C2,
-                       const float* chs2, const float* gamma, const float* beta, float eps, const float* emb, int emb_ld,
-                       const float* embz, int embz_ld, int silu, int B, int H, int W, void* out_act, void* out_raw,
-                       int raw_dtype, pdae_stream_t stream);
 /* Per-channel variant of the statistics (what the tensor-core conv epilogue accumulates): chs[b][c] = (sum, sum^2)
  * in fp32.  pdae_ch_stats fills it for a tensor that no conv epilogue produced; pdae_gn_coef_ch forms the 32 group
  * statistics over the virtual concat [chs1 | chs2] (groups may straddle the seam) and folds the affine / AdaGN terms. */
@@ -147,16 +138,6 @@ int pdae_mlp_mod_ln_act(const float* h, const float* cond, const float* ln_w, co
 /* dst[b][col0 + j] = src[b][j], j < N (row strides dst_ld / N).                                       */
 int pdae_copy_cols(const float* src, float* dst, int dst_ld, int col0, int B, int N, pdae_stream_t stream);
 
-/* ---- tensor-core convolution: TMA -> wgmma (bf16 x bf16 -> fp32 in registers) ---------------------
- * Same contract as pdae_conv2d_simt for ksize in {1,3}, stride 1, pad ksize/2, Cin % 64 == 0,
- * Cout % 64 == 0, bf16 NHWC input (already normalised/activated by pdae_gn_apply), weights bf16
- * [k*k][Cout][Cin].  A plan owns the TMA descriptors for fixed buffers; run it any number of times.   */
-typedef struct pdae_conv_tc_plan pdae_conv_tc_plan;
-int pdae_conv_tc_create(pdae_conv_tc_plan** plan, const void* in_bf16, const void* w_bf16, const float* bias,
-                        const float* residual, float* out, int B, int H, int W, int Cin, int Cout, int ksize);
-int pdae_conv_tc_run(const pdae_conv_tc_plan* plan, pdae_stream_t stream);
-void pdae_conv_tc_destroy(pdae_conv_tc_plan* plan);
-
 
 /* ---- backward (training config: autograd through module.py:278-297,361-384,422-428 and the encoders), fp32 ---------
  * dgrad: dx[B,H,W,Cin] (+)= conv^T(dy[B,Ho,Wo,Cout]); w_tco fp32 [k*k][Cout][Cin].
@@ -205,7 +186,8 @@ int pdae_gemm_batched_simt(const float* A, int64_t lda, int64_t a_bs, int64_t a_
  * sources, weights bf16 [9][Cout][Cin] (w_skip [Cout][S1+S2]).  src_dtype PDAE_F32 = split-operand mode: fp32 NHWC sources
  * are split hi/lo in the prologue, weights are (hi, lo) pairs [9][2][Cout][Cin] (w_skip [2][Cout][S1+S2]) and every
  * product is a_hi*W_hi + a_lo*W_hi + a_hi*W_lo (fp32-grade).  H % 16 == 0, W % 8 == 0, every channel count % 64 == 0
- * (pdae_conv_tc3_supported).  Residual / ch_stats / out_dtype as for v2; the fused skip conv's bias must be folded into `bias`. */
+ * (pdae_conv_tc3_supported).  Residual / ch_stats / out_dtype as for pdae_conv_tc2_create; the fused skip conv's bias must
+ * be folded into `bias`. */
 typedef struct pdae_conv_tc3_plan pdae_conv_tc3_plan;
 int pdae_conv_tc3_supported(int H, int W, int Cin, int Cout);
 int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan, const void* src1, int C1, const void* src2, int C2, int src_dtype,
@@ -228,7 +210,11 @@ int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan, const void* act3_bf16, const
 int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* plan, pdae_stream_t stream);
 void pdae_wgrad_tc_destroy(pdae_wgrad_tc_plan* plan);
 
-/* v2: persistent CTAs, two consumer warpgroups with register accumulators (the producer runs ahead into the next tile), TMA-store
+/* ---- tensor-core convolution: TMA -> wgmma (bf16 x bf16 -> fp32 in registers) ---------------------
+ * Same contract as pdae_conv2d_simt for ksize in {1,3}, stride 1, pad ksize/2, Cin % 64 == 0,
+ * Cout % 64 == 0, bf16 NHWC input (already normalised/activated by pdae_gn_apply), weights bf16
+ * [k*k][Cout][Cin].  A plan owns the TMA descriptors for fixed buffers; run it any number of times.
+ * Persistent CTAs, two consumer warpgroups with register accumulators (the producer runs ahead into the next tile), TMA-store
  * epilogue.  out_dtype PDAE_F32|PDAE_BF16; ch_stats (optional) fp32 [B][Cout][2] accumulates per-channel (sum, sum^2)
  * of the stored values (zero it first); a residual is read in the OUTPUT's dtype.  cout_valid > 0 selects the image-head variant:
  * Cout must be 16 (weights zero-padded), `out` is NCHW fp32 [B][cout_valid][H][W].  bn_override: 0 = auto.              */

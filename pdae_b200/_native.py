@@ -15,7 +15,7 @@ from typing import Optional
 _HERE = os.path.dirname(os.path.abspath(__file__))
 _ROOT = os.path.dirname(_HERE)
 LIB_PATH = os.path.join(_HERE, "libpdae_b200.so")
-SOURCES = ["conv_simt.cu", "norm_elementwise.cu", "attention_simt.cu", "conv_tc.cu", "conv_tc2.cu", "conv_tc3.cu", "wgrad_tc.cu", "plan_exec.cu", "backward_simt.cu", "train_io.cu"]
+SOURCES = ["conv_simt.cu", "norm_elementwise.cu", "attention_simt.cu", "conv_tc2.cu", "conv_tc3.cu", "wgrad_tc.cu", "plan_exec.cu", "backward_simt.cu", "train_io.cu"]
 
 PDAE_F32, PDAE_BF16 = 0, 1
 RESAMPLE_NONE, RESAMPLE_UP2, RESAMPLE_DOWN2 = 0, 1, 2
@@ -88,9 +88,6 @@ _SIGS = {
     "pdae_nchw_to_nhwc": (c_int, [_P, _P, c_int, c_int, c_int, _P]),
     "pdae_gemm_batched_simt": (c_int, [_P, c_int64, c_int64, c_int64, c_int, _P, c_int64, c_int64, c_int64, c_int, _P, c_int64,
                                        c_int64, c_int64, c_int, c_int, c_int, c_int, c_int, c_float, _P]),
-    "pdae_conv_tc_create": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
-    "pdae_conv_tc_run": (c_int, [_P, _P]),
-    "pdae_conv_tc_destroy": (None, [_P]),
     "pdae_conv_tc2_create": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, c_int,
                                      c_int, c_int]),
     "pdae_conv_tc2_create_skip": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, _P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int,
@@ -121,8 +118,6 @@ _SIGS = {
     "pdae_mul_mask_cols": (c_int, [_P, c_int, _P, c_float, c_int, c_int, _P]),
     "pdae_stem_conv_bf16": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_gn_apply_split3": (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P]),
-    "pdae_gn_norm_apply": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, _P, _P, _P, c_float, _P, c_int, _P, c_int, c_int, c_int,
-                                   c_int, c_int, _P, _P, c_int, _P]),
     "pdae_adam_ema_step": (c_int, [_P, _P, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_int64, c_float,
                                    c_float, _P]),
     "pdae_unpack_grads": (c_int, [_P, _P, c_int, c_int, _P, _P]),

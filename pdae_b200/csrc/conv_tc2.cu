@@ -639,12 +639,10 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
   pl->grid = a.tiles_total < g_num_sms ? a.tiles_total : g_num_sms;
   // Weights stationary in shared memory: when the whole layer's B operand fits beside >= 4 A-only stages and every CTA
   // runs several tiles of the single n-tile, the weights are fetched once per CTA instead of once per tile (the narrow
-  // 64-channel layers are L2->SM bandwidth-bound: this removes a third of their bytes).  PDAE_TC_WSTAT=0 disables (A/B aid).
-  static int wstat_env = -1;
-  if (wstat_env < 0) { const char* e = getenv("PDAE_TC_WSTAT"); wstat_env = (e && e[0] == '0') ? 0 : 1; }
+  // 64-channel layers are L2->SM bandwidth-bound: this removes a third of their bytes).
   int wbytes = 0;
   a.w_stat = 0;
-  if (wstat_env && !head && !d.w_batched && Cout == BN && b_bytes == BN * T2_BK * 2 && a.tiles_total >= 2 * pl->grid) {
+  if (!head && !d.w_batched && Cout == BN && b_bytes == BN * T2_BK * 2 && a.tiles_total >= 2 * pl->grid) {
     const int wb = total_all * b_bytes;
     if ((220 * 1024 - 1024 - staging - wb) / T2_A_BYTES >= 4) {
       a.w_stat = 1;

@@ -684,17 +684,6 @@ extern "C" int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan_out, const void* s
     if (sbw > T3_MAX_SB) sbw = T3_MAX_SB;
     if (sbw >= 3) { sa = 3; sb = sbw; }
   }
-  {   // tuning aids: force the halo / weight pipeline depths (if they fit)
-    const char* ea = getenv("PDAE_TC3_SA");
-    const char* eb = getenv("PDAE_TC3_SB");
-    if (ea && atoi(ea) >= 2 && atoi(ea) <= T3_MAX_SA) {
-      const int want = atoi(ea);
-      int sbw = (budget - want * a_stage) / b_bytes;
-      if (sbw > T3_MAX_SB) sbw = T3_MAX_SB;
-      if (sbw >= 2) { sa = want; sb = sbw; }
-    }
-    if (eb && atoi(eb) >= 2 && atoi(eb) <= sb) sb = atoi(eb);
-  }
   if (sb < 2) {
     delete pl;
     PDAE_REQUIRE(false, "conv_tc3_create: shared-memory budget too small (BN=%d x3=%d)", BN, (int)x3);

@@ -2,7 +2,6 @@
 // per-step diffusion arithmetic and the latent-MLP row op.  All HBM-bound: vectorised, coalesced along
 // the NHWC channel axis, one pass over the data each.
 #include <stdarg.h>
-#include <stdlib.h>
 
 #include "common.cuh"
 
@@ -302,77 +301,6 @@ __global__ void __launch_bounds__(256) gn_apply8_kernel(const TSrc* __restrict__
     a0 = *reinterpret_cast<const float4*>(pa); a1 = *reinterpret_cast<const float4*>(pa + 4);
     b0 = *reinterpret_cast<const float4*>(pb); b1 = *reinterpret_cast<const float4*>(pb + 4);
   }
-  __nv_bfloat16* po = out_act + (long long)b * HW * C + c;
-  TRaw* pr = out_raw ? out_raw + (long long)b * HW * C + c : nullptr;
-  const int stride = gridDim.x * ppc, pix0 = blockIdx.x * ppc + prow;
-  apply8_dispatch<TSrc, TSrc2, TRaw>(s1, C1, s2, C2, b, c, po, pr, C, pix0, stride, HW, a0, a1, b0, b1, silu);
-}
-
-// GroupNorm coefficients computed in the CTA prologue from the per-channel (sum, sum^2) the conv epilogues accumulated:
-// same arithmetic as gn_coef_ch_kernel (fp64 group moments -> fp32 mean / rstd -> fp32 affine), without the extra launch
-// and without the [B][2][C] coefficient round trip.  blockDim.x >= 64.
-struct GnNormArgs {
-  const float* chs1; const float* chs2;   // [B][C1][2], [B][C2][2]
-  const float* gamma; const float* beta;
-  const float* emb; const float* embz;    // this block's [scale | shift] row slices or nullptr
-  int emb_ld, embz_ld;
-  float eps;
-};
-template <typename TSrc, typename TSrc2, typename TRaw>
-__global__ void __launch_bounds__(256) gn_norm_apply8_kernel(const TSrc* __restrict__ s1, int C1, const TSrc2* __restrict__ s2,
-                                                             int C2, GnNormArgs g, int silu, int HW,
-                                                             __nv_bfloat16* __restrict__ out_act, TRaw* __restrict__ out_raw) {
-  __shared__ double gs[32][2];
-  __shared__ float gmean[32], grstd[32];
-  const int C = C1 + C2, L = C >> 3, cpg = C >> 5;
-  const int b = blockIdx.y;
-  if (threadIdx.x < 64) {
-    const int gi = threadIdx.x & 31, which = threadIdx.x >> 5;
-    double a = 0.0;
-    for (int j = 0; j < cpg; ++j) {
-      const int c = gi * cpg + j;
-      a += (double)(c < C1 ? g.chs1[((long long)b * C1 + c) * 2 + which] : g.chs2[((long long)b * C2 + (c - C1)) * 2 + which]);
-    }
-    gs[gi][which] = a;
-  }
-  __syncthreads();
-  if (threadIdx.x < 32) {
-    const double n = (double)HW * cpg;
-    const double mean = gs[threadIdx.x][0] / n;
-    double var = gs[threadIdx.x][1] / n - mean * mean;
-    var = var < 0.0 ? 0.0 : var;
-    grstd[threadIdx.x] = (float)(1.0 / sqrt(var + (double)g.eps));
-    gmean[threadIdx.x] = (float)mean;
-  }
-  __syncthreads();
-  const int cq = threadIdx.x % L, prow = threadIdx.x / L, ppc = blockDim.x / L;
-  const int c = cq * 8;
-  float av[8], bv[8];
-  {
-    const float4 g0 = *reinterpret_cast<const float4*>(g.gamma + c), g1 = *reinterpret_cast<const float4*>(g.gamma + c + 4);
-    const float4 e0 = *reinterpret_cast<const float4*>(g.beta + c), e1 = *reinterpret_cast<const float4*>(g.beta + c + 4);
-    const float gm[8] = {g0.x, g0.y, g0.z, g0.w, g1.x, g1.y, g1.z, g1.w};
-    const float bt[8] = {e0.x, e0.y, e0.z, e0.w, e1.x, e1.y, e1.z, e1.w};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const int gi = (c + j) / cpg;
-      av[j] = gm[j] * grstd[gi];
-      bv[j] = bt[j] - gmean[gi] * av[j];
-    }
-    auto mod = [&](const float* e, int ld) {   // AdaGN: h*(1+scale)+shift
-      const float* ps = e + (long long)b * ld + c;
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const float sc = 1.0f + ps[j], sh = ps[C + j];
-        av[j] *= sc;
-        bv[j] = bv[j] * sc + sh;
-      }
-    };
-    if (g.emb) mod(g.emb, g.emb_ld);
-    if (g.embz) mod(g.embz, g.embz_ld);
-  }
-  const float4 a0 = make_float4(av[0], av[1], av[2], av[3]), a1 = make_float4(av[4], av[5], av[6], av[7]);
-  const float4 b0 = make_float4(bv[0], bv[1], bv[2], bv[3]), b1 = make_float4(bv[4], bv[5], bv[6], bv[7]);
   __nv_bfloat16* po = out_act + (long long)b * HW * C + c;
   TRaw* pr = out_raw ? out_raw + (long long)b * HW * C + c : nullptr;
   const int stride = gridDim.x * ppc, pix0 = blockIdx.x * ppc + prow;
@@ -782,13 +710,7 @@ extern "C" int pdae_gn_apply(const void* src1, int src1_dtype, int C1, const voi
     const int L8 = (C1 + C2) / 8;
     const int ppc = 256 / L8;
     const int nthr = L8 * ppc;
-    static int ppt = 0;                   // pixels per thread (tuning aid: PDAE_APPLY_PPT)
-    if (ppt == 0) {
-      const char* e = getenv("PDAE_APPLY_PPT");
-      ppt = e ? atoi(e) : 8;
-      if (ppt < 1) ppt = 4;
-    }
-    int gx = cdiv(HW, ppc * ppt);        // several pixels per thread (unrolled x4) keep loads in flight
+    int gx = cdiv(HW, ppc * 8);          // 8 pixels per thread (unrolled x4) keep loads in flight
     if (gx > 148 * 16) gx = 148 * 16;
     if (gx < 1) gx = 1;
     dim3 grid(gx, B);
@@ -856,41 +778,6 @@ extern "C" int pdae_gn_apply_split3(const float* src1, int C1, const float* src2
   else PDAE_SPLIT3(PDAE_RESAMPLE_DOWN2);
 #undef PDAE_SPLIT3
   PDAE_LAUNCH_CHECK("gn_apply_split3_kernel");
-  return PDAE_OK;
-}
-
-extern "C" int pdae_gn_norm_apply(const void* src1, int src1_dtype, int C1, const float* chs1, const void* src2, int src2_dtype,
-                                  int C2, const float* chs2, const float* gamma, const float* beta, float eps, const float* emb,
-                                  int emb_ld, const float* embz, int embz_ld, int silu, int B, int H, int W, void* out_act,
-                                  void* out_raw, int raw_dtype, pdae_stream_t stream) {
-  PDAE_REQUIRE(src1 && chs1 && gamma && beta && out_act, "gn_norm_apply: null pointer");
-  if (!src2) { C2 = 0; src2_dtype = src1_dtype; }
-  PDAE_REQUIRE(C2 == 0 || chs2, "gn_norm_apply: second source without statistics");
-  const int C = C1 + C2;
-  PDAE_REQUIRE(C1 % 8 == 0 && C2 % 8 == 0 && C % 32 == 0 && C >= 64 && C / 8 <= 256,
-               "gn_norm_apply: C1=%d C2=%d unsupported (need multiples of 8, 64 <= C <= 2048, C %% 32 == 0)", C1, C2);
-  if (!out_raw) raw_dtype = PDAE_BF16;
-  GnNormArgs g{chs1, chs2, gamma, beta, emb, embz, emb_ld, embz_ld, eps};
-  const int HW = H * W, L8 = C / 8, ppc = 256 / L8, nthr = L8 * ppc;
-  int gx = cdiv(HW, ppc * 8);
-  if (gx > 148 * 16) gx = 148 * 16;
-  if (gx < 1) gx = 1;
-  dim3 grid(gx, B);
-  cudaStream_t s = (cudaStream_t)stream;
-  typedef __nv_bfloat16 bf;
-  const int key = src1_dtype | (src2_dtype << 1) | (raw_dtype << 2);
-  switch (key) {
-    case 0 | 0 | 0: gn_norm_apply8_kernel<float, float, float><<<grid, nthr, 0, s>>>((const float*)src1, C1, (const float*)src2, C2, g, silu, HW, (bf*)out_act, (float*)out_raw); break;
-    case 0 | 0 | 4: gn_norm_apply8_kernel<float, float, bf><<<grid, nthr, 0, s>>>((const float*)src1, C1, (const float*)src2, C2, g, silu, HW, (bf*)out_act, (bf*)out_raw); break;
-    case 1 | 2 | 0: gn_norm_apply8_kernel<bf, bf, float><<<grid, nthr, 0, s>>>((const bf*)src1, C1, (const bf*)src2, C2, g, silu, HW, (bf*)out_act, (float*)out_raw); break;
-    case 1 | 2 | 4: gn_norm_apply8_kernel<bf, bf, bf><<<grid, nthr, 0, s>>>((const bf*)src1, C1, (const bf*)src2, C2, g, silu, HW, (bf*)out_act, (bf*)out_raw); break;
-    case 1 | 0 | 0: gn_norm_apply8_kernel<bf, float, float><<<grid, nthr, 0, s>>>((const bf*)src1, C1, (const float*)src2, C2, g, silu, HW, (bf*)out_act, (float*)out_raw); break;
-    case 1 | 0 | 4: gn_norm_apply8_kernel<bf, float, bf><<<grid, nthr, 0, s>>>((const bf*)src1, C1, (const float*)src2, C2, g, silu, HW, (bf*)out_act, (bf*)out_raw); break;
-    case 0 | 2 | 0: gn_norm_apply8_kernel<float, bf, float><<<grid, nthr, 0, s>>>((const float*)src1, C1, (const bf*)src2, C2, g, silu, HW, (bf*)out_act, (float*)out_raw); break;
-    case 0 | 2 | 4: gn_norm_apply8_kernel<float, bf, bf><<<grid, nthr, 0, s>>>((const float*)src1, C1, (const bf*)src2, C2, g, silu, HW, (bf*)out_act, (bf*)out_raw); break;
-    default: PDAE_REQUIRE(false, "gn_norm_apply: unsupported dtype combination");
-  }
-  PDAE_LAUNCH_CHECK("gn_norm_apply8_kernel");
   return PDAE_OK;
 }
 

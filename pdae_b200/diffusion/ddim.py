@@ -8,7 +8,6 @@ allocation, no host sync, no tqdm).
 from __future__ import annotations
 
 import ctypes
-import os
 from functools import partial
 
 import numpy as np
@@ -41,8 +40,7 @@ def _t64(t, B, what):
 class _StepRunner:
     """One network plan + the loop bookkeeping + the fused update of a DDIM loop direction, replayed as ONE CUDA graph per
     step.  The graph is cached on the plan, keyed by (DDIM object, direction, shift) -- those fix the table pointers the
-    update kernel reads.  `seek(i)` sets the device-side step counter; `step()` is a single graph launch (or, with
-    PDAE_NO_GRAPH=1, the same launch sequence issued eagerly)."""
+    update kernel reads.  `seek(i)` sets the device-side step counter; `step()` is a single graph launch."""
 
     def __init__(self, ddim: "DDIM", plan, x_in, t_in, eps, grad, direction: str, C: int):
         self.d, self.plan, self.x_in, self.t_in, self.eps, self.grad, self.direction = ddim, plan, x_in, t_in, eps, grad, direction
@@ -86,7 +84,7 @@ class _StepRunner:
             d._update(x, self.ent["t_loc"], self.eps.tensor, self.grad.tensor if self.grad is not None else None,
                       self.direction, out=x)
 
-    def begin(self, use_graph: bool):
+    def begin(self):
         self.plan.run_prologue()          # forced weight re-pack + step-invariant ops (label_emb(z), emb_z_layers)
         # DDIM update fused into the last head conv's epilogue: point its device-side descriptor at this loop's tables
         fuse, is_grad_head = self._fuse_target()
@@ -104,7 +102,7 @@ class _StepRunner:
                     d.sqrt_one_minus_alphas_cumprod.data_ptr(), tab.data_ptr()]
             fuse.tensor.copy_(torch.tensor(desc, dtype=torch.int64))
         gkey = "graph_fused" if self.fused else "graph"
-        if use_graph and self.ent.get(gkey) is None:
+        if self.ent.get(gkey) is None:
             self.seek(1 if self.direction == "sample" else 0)
             self._launch_step()           # warm-up outside capture (lazy module loading, cudaFuncSetAttribute, ...)
             torch.cuda.synchronize(self.d.device)
@@ -112,8 +110,7 @@ class _StepRunner:
             with torch.cuda.graph(g):
                 self._launch_step()
             self.ent[gkey] = g
-        self.graph = self.ent.get(gkey)
-        self.use_graph = use_graph
+        self.graph = self.ent[gkey]
 
     def end(self):
         """Switch the fused update off again: the plan is shared with plain forward calls."""
@@ -124,10 +121,7 @@ class _StepRunner:
         self.ent["counter"].fill_(int(i))
 
     def step(self):
-        if self.use_graph:
-            self.graph.replay()
-        else:
-            self._launch_step()
+        self.graph.replay()
         if not self.in_graph_update:
             x = self.x_in.tensor
             e = self.eps.tensor[:, :self.C].contiguous()
@@ -135,9 +129,6 @@ class _StepRunner:
 
 
 class DDIM:
-    # replay each network step as one CUDA graph in the native fast path (PDAE_NO_GRAPH=1 disables, e.g. under ncu)
-    use_cuda_graph = os.environ.get("PDAE_NO_GRAPH", "0") != "1"
-
     def __init__(self, betas, timestep_map, device):
         self.device = device
         self.timestep_map = timestep_map.to(self.device)
@@ -230,9 +221,9 @@ class DDIM:
             if c_in is not None:
                 c_in.tensor.copy_(cond)
             main = _StepRunner(self, plan, x_in, t_in, eps, None, direction, C)
-        main.begin(self.use_cuda_graph)   # re-packs weights (forced: `.data` / raw-pointer updates bump no version), prologue
+        main.begin()   # re-packs weights (forced: `.data` / raw-pointer updates bump no version), prologue
         if tail is not None:
-            tail.begin(self.use_cuda_graph)
+            tail.begin()
         try:
             x_in.tensor.copy_(x)
             cur = main

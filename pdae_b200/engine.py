@@ -8,9 +8,12 @@ PyTorch is used here only for device memory and streams.
 Precision modes
   * ``fp32``: every contraction on CUDA cores in fp32 (pdae_conv2d_simt / pdae_attention_simt).  This is
     the mode that holds rtol 1e-3 / atol 1e-4 against the CPU oracle.
-  * ``bf16``: convolutions whose shape allows it run on the wgmma tensor-core kernel with bf16 operands
-    and fp32 accumulation (pdae_conv_tc_*); the residual stream, GroupNorm statistics, embeddings and
-    the DDIM update stay fp32.
+  * ``bf16``: convolutions and attention GEMMs whose shapes allow it run on the wgmma tensor-core kernels
+    with bf16 operands and fp32 accumulation (pdae_conv_tc2_* / pdae_gemm_tc2_*, and pdae_conv_tc3_* with
+    GroupNorm-apply / SiLU fused into the operand path); the residual stream is bf16, GroupNorm statistics,
+    embeddings and the DDIM update stay fp32.
+  * ``bf16x3``: the same tensor-core kernels on split operands (a = hi + lo, three bf16 products per term)
+    for fp32-grade results; the residual stream and GroupNorm inputs stay fp32.
 """
 from __future__ import annotations
 
@@ -130,15 +133,9 @@ class Plan:
             raise ValueError(f"precision must be one of {PRECISIONS}")
         self.x3 = self.precision == "bf16x3"                     # split-operand tensor-core mode (fp32-grade results)
         self.tc = self.precision in ("bf16", "bf16x3")
-        self.v2 = os.environ.get("PDAE_TC_V1", "0") != "1" or self.x3   # persistent v2 conv kernel (default) vs the simple v1
-        self.bn_override = int(os.environ.get("PDAE_TC_BN", "0"))  # tuning aid: force the N tile of the v2 kernel
         # residual stream (block outputs / skip tensors) kept in bf16 instead of fp32: halves the HBM bytes of the
-        # bandwidth-bound top-level layers.  "bf16" precision + v2 kernel only.
-        self.stream_bf16 = self.tc and self.v2 and not self.x3 and os.environ.get("PDAE_STREAM_BF16", "1") == "1"
-        # conv_tc3: GroupNorm-apply / AdaGN / SiLU (and the bf16x3 hi/lo split) fused into the conv's operand path -- the
-        # activated tensor never exists in HBM.  PDAE_TC3=0 restores the separate gn_apply + conv_tc2 pair (A/B aid).
-        self.fuse_prologue = self.tc and self.v2 and os.environ.get("PDAE_TC3", "1") == "1"
-        self.fuse_coef = os.environ.get("PDAE_FUSE_COEF", "0") == "1"   # GN coefficients inside gn_apply (A/B aid, off by default)
+        # bandwidth-bound top-level layers.  "bf16" precision only.
+        self.stream_bf16 = self.precision == "bf16"
         self.L = _native.lib()
         self.ops: List[Tuple[str, list]] = []
         # ops recorded inside `with P.prologue():` depend only on inputs that are constant over a sampling loop (z):
@@ -150,7 +147,6 @@ class Plan:
         self.params: List[Tuple[torch.Tensor, int]] = []
         self._pack_cache: Dict[tuple, Buf] = {}
         self._compiled = None
-        self._tc_handles: List[ctypes.c_void_p] = []
         self._tc2_handles: List[ctypes.c_void_p] = []
         self._tc3_handles: List[ctypes.c_void_p] = []
         self._wg_handles: List[ctypes.c_void_p] = []
@@ -296,9 +292,6 @@ class Plan:
                 free.append(b._block)  # type: ignore[attr-defined]
         compiled = []
         for fn, args in self.ops:
-            if fn == "conv_tc":
-                compiled.append(self._compile_tc(args))
-                continue
             if fn == "conv_tc2":
                 compiled.append(self._compile_tc2(args))
                 continue
@@ -347,15 +340,6 @@ class Plan:
         if isinstance(a, BufView):
             return ctypes.c_void_p(a.buf.tensor.data_ptr() + a.off * a.buf.tensor.element_size())
         return a
-
-    def _compile_tc(self, args):
-        x, w, bias, resid, out, B, H, W, Cin, Cout, k = args
-        h = ctypes.c_void_p()
-        rc = self.L.pdae_conv_tc_create(ctypes.byref(h), self._resolve(x), self._resolve(w), self._resolve(bias),
-                                        self._resolve(resid), self._resolve(out), B, H, W, Cin, Cout, k)
-        _native.check(rc, "pdae_conv_tc_create")
-        self._tc_handles.append(h)
-        return (self.L.pdae_conv_tc_run, [h, None], 1, "conv_tc")
 
     def _compile_tc2(self, args):
         fuse = args[15] if len(args) > 15 else None
@@ -439,17 +423,14 @@ class Plan:
                   flops=2.0 * batch * M * N * K if flops is None else flops)
 
     def can_gemm_tc(self, M: int, N: int, K: int) -> bool:
-        return self.tc and self.v2 and not self.x3 and M % 128 == 0 and N % 64 == 0 and K % 64 == 0
+        return self.tc and not self.x3 and M % 128 == 0 and N % 64 == 0 and K % 64 == 0
 
     def can_gemm_x3(self, M: int, N: int, K: int) -> bool:
         """Batched GEMM in the split-operand mode: K is the LOGICAL depth (the operand blocks hold 3*K)."""
-        return self.x3 and self.v2 and M % 128 == 0 and N % 64 == 0 and K % 64 == 0 and \
-            os.environ.get("PDAE_X3_ATTN_TC", "1") == "1"
+        return self.x3 and M % 128 == 0 and N % 64 == 0 and K % 64 == 0
 
     def __del__(self):
         try:
-            for h in self._tc_handles:
-                self.L.pdae_conv_tc_destroy(h)
             for h in self._tc2_handles:
                 self.L.pdae_conv_tc2_destroy(h)
             for h in self._tc3_handles:
@@ -567,8 +548,6 @@ class Plan:
     def _tc_shape_ok(self, Cin: int, Cout: int, k: int, stride: int, H: int, W: int) -> bool:
         if stride != 1 or k not in (1, 3) or Cin % 64 or Cout % 64:
             return False
-        if not self.v2 and ((H & (H - 1)) or (W & (W - 1))):
-            return False   # the legacy v1 kernel (PDAE_TC_V1=1, A/B aid) only tiles power-of-two images
         tw = 1
         while tw * 2 <= 128 and W % (tw * 2) == 0:
             tw *= 2
@@ -594,7 +573,7 @@ class Plan:
             wp = self.pack((wkey or id(weight), "tc_x3"), [weight],
                            lambda Cin=Cin: split3_weights(weight.detach().reshape(Cout, Cin, k * k)))
             self.call("conv_tc2", x3b, wp, self.param(bias), residual, out, PDAE_F32, None, B, H, W, 3 * Cin, Cout, k, 0,
-                      bn_override or self.bn_override, flops=2.0 * B * H * W * Cout * Cin * k * k)
+                      bn_override, flops=2.0 * B * H * W * Cout * Cin * k * k)
             return None
         bias_b = self.param(bias)
         wkey = wkey or id(weight)
@@ -608,10 +587,6 @@ class Plan:
             else:
                 wp = self.pack((wkey, "tc"), [weight],
                                lambda: wsrc().reshape(Cout, Cin, k * k).permute(2, 0, 1).to(torch.bfloat16))
-            if not self.v2:
-                assert out.dtype == torch.float32
-                self.call("conv_tc", x, wp, bias_b, residual, out, B, H, W, Cin, Cout, k, flops=fl)
-                return None
             stats = self.new_stats(B, Cout) if want_stats else None
             if skip is not None:
                 # fused 1x1 skip conv (model/module.py:268-276): extra K blocks accumulated into the same accumulator tile
@@ -630,10 +605,10 @@ class Plan:
                 bsum = self.pack((id(bias), id(sb), "bias_sum"), [bias, sb], lambda: (bias.detach() + sb.detach()).float())
                 self.params.append((sb, sb.data_ptr()))
                 self.call("conv_tc2_skip", x, wp, bsum, sk_in, w2, Cin2, out, _DT[out.dtype], stats, B, H, W, Cin, Cout, k,
-                          bn_override or self.bn_override, flops=fl + 2.0 * B * H * W * Cout * (Cin2 // 3 if x3 else Cin2))
+                          bn_override, flops=fl + 2.0 * B * H * W * Cout * (Cin2 // 3 if x3 else Cin2))
                 return stats
             self.call("conv_tc2", x, wp, bias_b, residual, out, _DT[out.dtype], stats, B, H, W, Cin, Cout, k, 0,
-                      bn_override or self.bn_override, flops=fl)
+                      bn_override, flops=fl)
             return stats
         assert out.dtype == torch.float32, "CUDA-core conv writes fp32"
         wp = self.pack((wkey, "simt"), [weight], lambda: weight.detach().reshape(Cout, Cin, k * k).permute(2, 1, 0).float())
@@ -646,7 +621,7 @@ class Plan:
     def can_fuse_prologue(self, srcs: Sequence[Tuple[Optional[Buf], int]], Cout: int, H: int, W: int) -> bool:
         """3x3 stride-1 conv whose input is SiLU(a*x+b) of (a virtual concat of) NHWC tensors already in this mode's
         stream dtype: 16 x 8 output tiles of one image, 64-channel k-blocks that do not straddle the concat seam."""
-        if not self.fuse_prologue or H % 16 or W % 8 or Cout % 64:
+        if not self.tc or H % 16 or W % 8 or Cout % 64:
             return False
         want = torch.float32 if self.x3 else torch.bfloat16
         for b, C in srcs:
@@ -707,7 +682,7 @@ class Plan:
             bias_b = self.param(bias)
         stats = self.new_stats(B, Cout) if want_stats else None
         self.call("conv_tc3", s1, C1, s2, C2, PDAE_F32 if x3 else PDAE_BF16, ab, int(silu), wp, bias_b, k1, S1, k2, S2, wsk,
-                  residual, out, _DT[out.dtype], stats, B, H, W, Cout, bn_override or self.bn_override, flops=fl)
+                  residual, out, _DT[out.dtype], stats, B, H, W, Cout, bn_override, flops=fl)
         return stats
 
     def linear(self, x: Buf, weight: torch.Tensor, bias: Optional[torch.Tensor], out: Buf, *, B, Cin, Cout, a_silu=False,
@@ -725,7 +700,7 @@ class Plan:
         device-side descriptor through which a sampling loop can switch on the DDIM update fused into this head's epilogue
         (Plan.head_fuse[fuse_key]; all-zero = plain head)."""
         fl = 2.0 * B * H * W * Cout * Cin * 9
-        if self.v2 and x.dtype == torch.bfloat16 and Cout <= 16 and self.use_tc(Cin, 64, 3, 1, H, W):
+        if x.dtype == torch.bfloat16 and Cout <= 16 and self.use_tc(Cin, 64, 3, 1, H, W):
             # tensor-core head: Cout zero-padded to one 16-wide UMMA tile, NCHW fp32 planes written by the epilogue
             x3 = bool(x.split3)
             Ce = 3 * Cin if x3 else Cin
@@ -738,7 +713,7 @@ class Plan:
                 return z
             wp = self.pack((id(weight), "tc16_x3" if x3 else "tc16"), [weight], pack16)
             fuse = None
-            if fuse_key is not None and os.environ.get("PDAE_HEAD_FUSE", "1") == "1":
+            if fuse_key is not None:
                 with torch.inference_mode(False):
                     fuse = self.fixed(torch.zeros(8, dtype=torch.int64, device=self.device))
                 self.head_fuse[fuse_key] = fuse
@@ -761,7 +736,7 @@ class Plan:
         """dtype the normalised input of an image-head conv should be produced in (bf16 only if a bf16 kernel takes it)."""
         if not self.tc:
             return torch.float32
-        if self.v2 and Cout <= 16 and self.use_tc(Cin, 64, 3, 1, H, W):
+        if Cout <= 16 and self.use_tc(Cin, 64, 3, 1, H, W):
             return torch.bfloat16
         if Cout <= 4 and Cin % 4 == 0 and not self.x3:      # CUDA-core small-N head: plain bf16 input (fp32 in the x3 mode)
             return torch.bfloat16
@@ -781,7 +756,7 @@ class Plan:
 
     @property
     def fused_stats(self) -> bool:
-        return self.tc and self.v2
+        return self.tc
 
     @property
     def stream_dtype(self):
@@ -796,7 +771,7 @@ class Plan:
 
     def gn_coef(self, src1: Buf, C1: int, src2: Optional[Buf], C2: int, gamma, beta, *, B, HW, emb=None, emb_ld=0,
                 embz=None, embz_ld=0, stats1: Optional[Buf] = None, stats2: Optional[Buf] = None) -> Buf:
-        """GroupNorm(32) statistics -> per-(b,c) affine coefficients.  bf16/v2 mode consumes the per-channel sums the
+        """GroupNorm(32) statistics -> per-(b,c) affine coefficients.  The tensor-core modes consume the per-channel sums the
         conv epilogues accumulated (computing missing ones); fp32 mode keeps the fp64 two-kernel path."""
         C = C1 + C2
         if self.fused_stats:
@@ -804,7 +779,7 @@ class Plan:
                 stats1 = self.ch_stats(src1, C1, B=B, HW=HW)
             if src2 is not None and stats2 is None:
                 stats2 = self.ch_stats(src2, C2, B=B, HW=HW)
-            # deferred: gn_apply folds the coefficient computation into its own launch when its kernel allows it
+            # deferred: the consumer (gn_apply / conv_fused) launches gn_coef_ch right before the op that reads them
             return CoefSpec(stats1, C1, stats2, C2, self.param(gamma), self.param(beta), B, HW, emb, emb_ld, embz, embz_ld)
         ab = self.new((B, 2, C), torch.float32, "gn_ab")
         sums = self.new((B, 32, 2), torch.float64, "gn_sums")
@@ -838,13 +813,6 @@ class Plan:
         raw = self.new((B, Ho, Wo, C), raw_dtype, "raw") if raw_dtype is not None else None
         if isinstance(ab, CoefSpec):
             c = ab
-            if (self.fuse_coef and resample == RESAMPLE_NONE and act_dtype == torch.bfloat16 and C1 % 8 == 0 and C2 % 8 == 0
-                    and 64 <= C <= 2048):
-                self.call("gn_norm_apply", src1, _DT[src1.dtype], C1, c.stats1, src2,
-                          _DT[src2.dtype] if src2 is not None else PDAE_F32, C2, c.stats2, c.gamma, c.beta, ctypes.c_float(1e-5),
-                          c.emb, c.emb_ld, c.embz, c.embz_ld, int(silu), B, H, W, act, raw,
-                          _DT[raw_dtype] if raw_dtype is not None else PDAE_F32, _STREAM)
-                return act, raw
             ab = self.new((B, 2, C), torch.float32, "gn_ab")
             self.call("gn_coef_ch", c.stats1, c.C1, c.stats2, c.C2, c.gamma, c.beta, c.B, c.HW, ctypes.c_float(1e-5),
                       c.emb, c.emb_ld, c.embz, c.embz_ld, ab, _STREAM)

@@ -12,7 +12,6 @@ against the reference keep working; activations inside a plan are NHWC.
 from __future__ import annotations
 
 import ctypes
-import os
 import math
 from typing import Dict, Optional, Tuple
 
@@ -317,10 +316,9 @@ class _ResBase(PlannedModule):
         plain = not self.updown and x.b2 is None        # x.b1 itself is the skip-path input
         # a concatenated input whose 1x1 skip conv is folded into conv2 is read from its two source tensors directly
         # (two TMA maps): the concat is never materialised
-        cat_skip = (not ident and not self.updown and x.b2 is not None and P.v2 and tcs and tc2
+        cat_skip = (not ident and not self.updown and x.b2 is not None and tcs and tc2
                     and self.skip_connection.kernel_size[0] == 1 and x.b1.dtype == torch.bfloat16
-                    and x.b2.dtype == torch.bfloat16 and x.C1 % 64 == 0 and x.C2 % 64 == 0 and tape is None
-                    and os.environ.get("PDAE_CAT_SKIP", "1") == "1")
+                    and x.b2.dtype == torch.bfloat16 and x.C1 % 64 == 0 and x.C2 % 64 == 0 and tape is None)
         raw_dtype = None
         if cat_skip:
             pass
@@ -333,7 +331,7 @@ class _ResBase(PlannedModule):
                 raw_dtype = want
         act1, raw = P.gn_apply(x.b1, x.C1, x.b2, x.C2, ab1, silu=True, resample=rs, B=B, H=H, W=W,
                                act_dtype=torch.bfloat16 if tc1 else torch.float32, raw_dtype=raw_dtype)
-        # h only feeds GroupNorm-2: with the v2 kernel it is stored in bf16 and its statistics come from the epilogue
+        # h only feeds GroupNorm-2: on the tensor cores it is stored in bf16 and its statistics come from the epilogue
         h_bf16 = tc1 and P.fused_stats and not P.x3     # (the split-operand mode keeps every conv output in fp32)
         h = P.new((B, H2, W2, Co), torch.bfloat16 if h_bf16 else torch.float32, "res_h")
         hs = P.conv(act1, conv1.weight, conv1.bias, h, B=B, H=H2, W=W2, Cin=C, Cout=Co, k=3, want_stats=True)
@@ -360,7 +358,7 @@ class _ResBase(PlannedModule):
         else:
             sk = self.skip_connection
             sk_in = (x.b1, x.C1, x.b2, x.C2) if cat_skip else (raw if raw is not None else x.b1)
-            if cat_skip or (P.v2 and tcs and tc2 and sk.kernel_size[0] == 1 and sk_in.dtype == torch.bfloat16):
+            if cat_skip or (tcs and tc2 and sk.kernel_size[0] == 1 and sk_in.dtype == torch.bfloat16):
                 resid, fused_skip = None, (sk_in, sk.weight, sk.bias, C)   # folded into conv2 as extra K blocks
             else:
                 resid = P.new((B, H2, W2, Co), out_dt, "res_skip")
@@ -480,7 +478,7 @@ class AttentionBlock(PlannedModule):
             hs_ = 3 * ch if legacy else ch                  # channel stride between heads inside a qkv row
             ko = ch if legacy else C                        # offset of K relative to Q
             alpha = 1.0 / math.sqrt(ch)                     # scale = ch^(-1/4) on both q and k (module.py:449-453)
-            fuse_sm = T in (64, 128, 256) and os.environ.get("PDAE_FUSE_SOFTMAX", "1") == "1"
+            fuse_sm = T in (64, 128, 256)
             S = None if fuse_sm else P.new((B * heads, T, T), torch.float32, "att_scores")
             for h in range(heads):
                 if fuse_sm:   # a whole score row sits in one accumulator tile: softmax in the GEMM epilogue

@@ -16,7 +16,6 @@ from __future__ import annotations
 
 import ctypes
 import math
-import os
 from typing import Callable, Dict, List, Optional, Tuple
 
 import numpy as np
@@ -105,9 +104,8 @@ def draw_dropout_masks(plan: Plan) -> None:
 def bwd_plan(dev) -> Plan:
     """Backward plans are split-operand tensor-core plans: the data gradient of every eligible stride-1 conv runs on
     `conv_tc2` and its weight gradient on `wgrad_tc`, both in the fp32-grade "bf16x3" mode (Backward.conv); everything else
-    in them is fp32 CUDA-core arithmetic.  PDAE_TRAIN_TC_DGRAD=0 selects pure fp32 CUDA-core backward plans (A/B aid: 176 vs
-    127 ms per celeba64-proxy step at B=32 in round 1; both pass the same gradient checks of tests/test_gpu_training.py)."""
-    return Plan(dev, "bf16x3" if os.environ.get("PDAE_TRAIN_TC_DGRAD", "1") == "1" else "fp32")
+    in them is fp32 CUDA-core arithmetic."""
+    return Plan(dev, "bf16x3")
 
 
 class Backward:
@@ -117,8 +115,6 @@ class Backward:
         self.P = BP
         self.sink = sink
         self._fixed: Dict[int, Buf] = {}
-        self.tc_dgrad = bool(getattr(BP, "x3", False))
-        self.tc_wgrad = self.tc_dgrad and os.environ.get("PDAE_TRAIN_TC_WGRAD", "1") == "1"
 
     def fx(self, b):
         if b is None:
@@ -144,7 +140,7 @@ class Backward:
         dy3 = None
         if trainable:
             dw = P.new_zeroed(kk * Cin * Cout)
-            if self.tc_wgrad and same and not a_silu and P.L.pdae_wgrad_tc_supported(H, W, Cin, Cout, k):
+            if same and not a_silu and P.L.pdae_wgrad_tc_supported(H, W, Cin, Cout, k):
                 # weight gradient on the tensor cores (wgrad_tc.cu): both operands split [hi | lo | hi], fp32-grade products
                 a3 = getattr(x, "split3_copy", None)       # left by the tensor-core training forward (Plan.conv, train_tc)
                 if a3 is not None and tuple(a3.shape) == (B, H, W, 3 * Cin):
@@ -156,8 +152,6 @@ class Backward:
                                     act_dtype=torch.bfloat16)
                 P.call("wgrad_tc", a3, dy3, dw, B, H, W, Cin, Cout, k, flops=2.0 * B * H * W * Cin * Cout * kk)
             else:
-                if os.environ.get("PDAE_TRAIN_DEBUG") == "1":
-                    print(f"[train] CUDA-core wgrad: B{B} {H}x{W} {Cin}->{Cout} k{k} s{stride} nchw{int(in_nchw)} silu{int(a_silu)}")
                 P.call("conv2d_wgrad_simt", self.fx(x), int(in_nchw), int(a_silu), dy, dw, B, H, W, Cin, Cout, k, stride, pad,
                        _STREAM)
             unpack = w_unpack or (lambda t, kk=kk, Cin=Cin, Cout=Cout: t.view(kk, Cin, Cout).permute(2, 1, 0))
@@ -168,7 +162,7 @@ class Backward:
                 self.sink.add(bias, db, Cout, lambda t: t)
         if not need_dx:
             return None
-        if self.tc_dgrad and same and P.use_tc(Cout, Cin, k, 1, H, W):
+        if same and P.use_tc(Cout, Cin, k, 1, H, W):
             # dgrad of a stride-1 "same" conv = conv of dy with the transposed, spatially flipped weights: on the tensor
             # cores in the split-operand (fp32-grade) mode -- dy is split [hi | lo | hi], W' packed [W'_hi | W'_hi | W'_lo]
             if dy3 is None:
@@ -178,8 +172,6 @@ class Backward:
             P.conv(dy3, weight, None, dx, B=B, H=H, W=W, Cin=Cout, Cout=Cin, k=k, wkey=(id(weight), "dgrad"),
                    w_transform=lambda w, Cout=Cout, Cin=Cin, k=k: w.reshape(Cout, Cin, k, k).flip(2, 3).transpose(0, 1).contiguous())
             return dx
-        if os.environ.get("PDAE_TRAIN_DEBUG") == "1":
-            print(f"[train] CUDA-core dgrad: B{B} {H}x{W} {Cin}->{Cout} k{k} s{stride} nchw{int(in_nchw)}")
         wt = P.pack((id(weight), "tco"), [weight], lambda: weight.detach().reshape(Cout, Cin, kk).permute(2, 0, 1).float())
         dx = P.new((B, H, W, Cin), torch.float32, "dx")
         P.call("conv2d_dgrad_simt", dy, wt, dx, B, H, W, Cin, Cout, k, stride, pad, 0, _STREAM)
@@ -343,74 +335,42 @@ class ShiftUNetTrainer(_Generation):
         # The FROZEN half (input / middle / output blocks, `out` head: 55 % of the forward FLOPs) builds no autograd graph in
         # the reference either (its parameters do not require grad): it runs as a tensor-core plan in the split-operand
         # (fp32-grade) mode with the fused-prologue convs, exactly like sampling; only its skip tensors and bottleneck output
-        # are handed to the trainable half.  PDAE_TRAIN_TC_FWD=0 restores the single fp32 CUDA-core forward plan (A/B aid).
-        tc_fwd = os.environ.get("PDAE_TRAIN_TC_FWD", "1") == "1"
-        self.frozen = None
-        if tc_fwd:
-            Fp = Plan(dev, "bf16x3")
-            self.x_in = Fp.new((B, net.input_channel, H, W), torch.float32, "x_nchw")
-            self.t_in = Fp.new((B,), torch.int64, "t")
-            self.x_in.keep = self.t_in.keep = True
-            emb_f = emit_time_embed(Fp, net.time_embed, self.t_in, B, base, E, dev)
-            bank_f = EmbBank(Fp, frozen_blocks, "t", emb_f, B, E, "train_t_frozen")
-            hf = emit_stem(Fp, net.input_blocks[0][0], self.x_in, B, H, W, net.input_channel)
-            hs_f = [hf]
-            for stage in list(net.input_blocks)[1:]:
-                hf = stage.emit(Fp, hf, bank_f)
-                hs_f.append(hf)
-            for sfrc in hs_f:                      # consumed by the trainable half's plan: private storage
-                sfrc.b1.keep = True
-            eps_h = net.middle_block.emit(Fp, hf, bank_f)
-            for stage, skip in zip(net.output_blocks, reversed(hs_f)):
-                eps_h = stage.emit(Fp, eps_h.cat(skip), bank_f)
-            self.eps = Fp.new((B, net.output_channel, H, W), torch.float32, "eps_nchw")
-            self.eps.keep = True
-            emit_head(Fp, net.out, eps_h, self.eps)
-            Fp.finalize()
-            self.frozen = Fp
+        # are handed to the trainable half.
+        Fp = Plan(dev, "bf16x3")
+        self.x_in = Fp.new((B, net.input_channel, H, W), torch.float32, "x_nchw")
+        self.t_in = Fp.new((B,), torch.int64, "t")
+        self.x_in.keep = self.t_in.keep = True
+        emb_f = emit_time_embed(Fp, net.time_embed, self.t_in, B, base, E, dev)
+        bank_f = EmbBank(Fp, frozen_blocks, "t", emb_f, B, E, "train_t_frozen")
+        hf = emit_stem(Fp, net.input_blocks[0][0], self.x_in, B, H, W, net.input_channel)
+        hs_f = [hf]
+        for stage in list(net.input_blocks)[1:]:
+            hf = stage.emit(Fp, hf, bank_f)
+            hs_f.append(hf)
+        for sfrc in hs_f:                      # consumed by the trainable half's plan: private storage
+            sfrc.b1.keep = True
+        eps_h = net.middle_block.emit(Fp, hf, bank_f)
+        for stage, skip in zip(net.output_blocks, reversed(hs_f)):
+            eps_h = stage.emit(Fp, eps_h.cat(skip), bank_f)
+        self.eps = Fp.new((B, net.output_channel, H, W), torch.float32, "eps_nchw")
+        self.eps.keep = True
+        emit_head(Fp, net.out, eps_h, self.eps)
+        Fp.finalize()
+        self.frozen = Fp
         P = Plan(dev, "fp32")
         P.keep_all = True
-        P.train_tc = tc_fwd       # trainable half: fp32 activations kept for the backward, convs on the tensor cores (split operands)
-        if tc_fwd:
-            t_src = P.fixed(self.t_in.tensor)
-        else:
-            self.x_in = P.new((B, net.input_channel, H, W), torch.float32, "x_nchw")
-            self.t_in = P.new((B,), torch.int64, "t")
-            t_src = self.t_in
+        P.train_tc = True         # trainable half: fp32 activations kept for the backward, convs on the tensor cores (split operands)
         self.z_in = P.new((B, net.latent_dim), torch.float32, "z")
-        emb = emit_time_embed(P, net.time_embed, t_src, B, base, E, dev)
+        emb = emit_time_embed(P, net.time_embed, P.fixed(self.t_in.tensor), B, base, E, dev)
         shift_emb = P.new((B, E), torch.float32, "shift_emb")
         P.linear(self.z_in, net.label_emb.weight, net.label_emb.bias, shift_emb, B=B, Cin=net.latent_dim, Cout=E)
         bank_t = EmbBank(P, shift_blocks, "t", emb, B, E, "train_t_shift")
         bank_z = EmbBank(P, shift_blocks, "z", shift_emb, B, E, "train_z_shift")
         tape: list = []
-        if tc_fwd:
-            hs = [Src(P.fixed(sfrc.b1.tensor), sfrc.C, B, sfrc.H, sfrc.W) for sfrc in hs_f]
-            h = hs[-1]
-            emb_of = bank_t
-            shift_h = net.shift_middle_block.emit(P, h, emb_of, bank_z, tape=tape)
-            for shift_stage in net.shift_output_blocks:
-                shift_h = shift_stage.emit(P, shift_h.cat(hs.pop()), emb_of, bank_z, tape=tape)
-        else:
-            bank_f = EmbBank(P, frozen_blocks, "t", emb, B, E, "train_t_frozen")
-            emb_of = lambda blk: (bank_t if id(blk) in bank_t.offsets else bank_f)(blk)
-            stem = net.input_blocks[0][0]
-            c0 = stem.weight.shape[0]
-            h0 = P.new((B, H, W, c0), torch.float32, "stem")
-            P.conv(self.x_in, stem.weight, stem.bias, h0, B=B, H=H, W=W, Cin=net.input_channel, Cout=c0, k=3, in_nchw=True)
-            h = Src(h0, c0, B, H, W)
-            hs = [h]
-            for stage in list(net.input_blocks)[1:]:
-                h = stage.emit(P, h, emb_of)
-                hs.append(h)
-            eps_h = net.middle_block.emit(P, h, emb_of)
-            shift_h = net.shift_middle_block.emit(P, h, emb_of, bank_z, tape=tape)
-            for stage, shift_stage in zip(net.output_blocks, net.shift_output_blocks):
-                skip = hs.pop()
-                eps_h = stage.emit(P, eps_h.cat(skip), emb_of)
-                shift_h = shift_stage.emit(P, shift_h.cat(skip), emb_of, bank_z, tape=tape)
-            self.eps = P.new((B, net.output_channel, H, W), torch.float32, "eps_nchw")
-            emit_head(P, net.out, eps_h, self.eps)
+        hs = [Src(P.fixed(sfrc.b1.tensor), sfrc.C, B, sfrc.H, sfrc.W) for sfrc in hs_f]
+        shift_h = net.shift_middle_block.emit(P, hs[-1], bank_t, bank_z, tape=tape)
+        for shift_stage in net.shift_output_blocks:
+            shift_h = shift_stage.emit(P, shift_h.cat(hs.pop()), bank_t, bank_z, tape=tape)
         self.grad = P.new((B, net.input_channel, H, W), torch.float32, "shift_nchw")
         emit_head(P, net.shift_out, shift_h, self.grad, tape=tape)
         P.finalize()
@@ -447,15 +407,14 @@ class ShiftUNetTrainer(_Generation):
         self.params = [p for m in net._shift_parts() for p in m.parameters()]
 
     def stale(self) -> bool:
-        return self.fwd.stale() or self.bwd.stale() or (self.frozen is not None and self.frozen.stale())
+        return self.fwd.stale() or self.bwd.stale() or self.frozen.stale()
 
     def forward(self, x, t, z):
         draw_dropout_masks(self.fwd)
         self.x_in.tensor.copy_(x)
         self.t_in.tensor.copy_(t)
         self.z_in.tensor.copy_(z)
-        if self.frozen is not None:
-            self.frozen.run()
+        self.frozen.run()
         self.fwd.run()
         return self.eps.tensor.clone(), self.grad.tensor.clone()
 
@@ -508,7 +467,7 @@ class UNetTrainer(_Generation):
         dev = net._device()
         P = Plan(dev, "fp32")
         P.keep_all = True
-        P.train_tc = os.environ.get("PDAE_TRAIN_TC_FWD", "1") == "1"   # convs on the tensor cores (split operands), fp32 activations kept
+        P.train_tc = True         # convs on the tensor cores (split operands), fp32 activations kept
         E, base, Cimg = net.time_embed_dim, net.base_channel, net.input_channel
         self.x_in = P.new((B, Cimg, H, W), torch.float32, "x_nchw")
         self.t_in = P.new((B,), torch.int64, "t")

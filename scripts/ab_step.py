@@ -1,5 +1,5 @@
-"""Graph-replay time of one ShiftUNet decoder step under the current env knobs (A/B aid: run variants as separate
-processes on the SAME box, alternating).  usage: [ENV=..] python scripts/ab_step.py [workload] [batch] [reps] [precision]"""
+"""Graph-replay time of one ShiftUNet decoder step at a given precision.
+usage: python scripts/ab_step.py [workload] [batch] [reps] [precision]"""
 import os
 import sys
 
@@ -41,5 +41,4 @@ for _ in range(3):
     ms = e0.elapsed_time(e1) / reps
     best = min(best, ms)
     tot += ms / 3
-knobs = {k: v for k, v in os.environ.items() if k.startswith("PDAE_")}
-print(f"ab_step {wl} B={B} {prec}: {tot:.3f} ms/step avg, {best:.3f} best, {plan.n_launch} launches  {knobs}")
+print(f"ab_step {wl} B={B} {prec}: {tot:.3f} ms/step avg, {best:.3f} best, {plan.n_launch} launches")

@@ -1,5 +1,5 @@
 """Time conv_tc3 (fused-prologue conv) in isolation through the C-ABI, rotating over several buffer sets (L2-cold-ish).
-usage: python scripts/conv3_bench.py B H W C1 C2 Cout x3(0/1) res(0/1) skip(0/1) [bn]      (env knobs: PDAE_TC3_SA / PDAE_TC3_SB)"""
+usage: python scripts/conv3_bench.py B H W C1 C2 Cout x3(0/1) res(0/1) skip(0/1) [bn]"""
 import ctypes
 import os
 import sys
@@ -52,5 +52,5 @@ e1.record()
 torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / (reps * nset)
 fl = 2.0 * B * H * W * Cout * (Cin * 9 + (Cin if skip else 0))
-print(f"conv_tc3 {B}x{H}x{W} {C1}+{C2}->{Cout} x3={x3} res={res} skip={skip} bn={bn} SA={os.environ.get('PDAE_TC3_SA', '-')} "
-      f"SB={os.environ.get('PDAE_TC3_SB', '-')}: {ms * 1e3:.1f} us  {fl / ms / 1e9:.1f} TFLOP/s (algorithmic)")
+print(f"conv_tc3 {B}x{H}x{W} {C1}+{C2}->{Cout} x3={x3} res={res} skip={skip} bn={bn}: "
+      f"{ms * 1e3:.1f} us  {fl / ms / 1e9:.1f} TFLOP/s (algorithmic)")

@@ -1,5 +1,5 @@
 """Time one tensor-core conv in isolation (L2-cold between reps by rotating over several buffer sets).
-usage: python scripts/conv_bench.py B H W Cin Cout k res(0/1) out_bf16(0/1) stats(0/1) [bn] [v1]"""
+usage: python scripts/conv_bench.py B H W Cin Cout k res(0/1) out_bf16(0/1) stats(0/1) [bn]"""
 import os
 import sys
 
@@ -10,7 +10,6 @@ from pdae_b200.engine import Plan
 
 B, H, W, Cin, Cout, k, res, obf, stats = (int(a) for a in sys.argv[1:10])
 bn = int(sys.argv[10]) if len(sys.argv) > 10 else 0
-v1 = len(sys.argv) > 11 and sys.argv[11] == "v1"
 dev = torch.device("cuda")
 nset = 4
 plans = []
@@ -18,7 +17,6 @@ w = (torch.randn(Cout, Cin, k, k, device=dev) / (Cin * k * k) ** 0.5)
 bias = torch.randn(Cout, device=dev)
 for i in range(nset):
     P = Plan(dev, "bf16")
-    P.v2 = not v1
     x = torch.randn(B, H, W, Cin, device=dev).to(torch.bfloat16)
     out = P.new((B, H, W, Cout), torch.bfloat16 if obf else torch.float32)
     out.keep = True
@@ -40,5 +38,5 @@ torch.cuda.synchronize()
 ms = e0.elapsed_time(e1) / (reps * nset)
 fl = 2.0 * B * H * W * Cout * Cin * k * k
 byts = B * H * W * (Cin * 2 + Cout * (2 if obf else 4) + (Cout * 4 if res else 0))
-print(f"conv {B}x{H}x{W} {Cin}->{Cout} k{k} res={res} obf16={obf} stats={stats} bn={bn} v1={v1}: {ms * 1e3:.1f} us  "
+print(f"conv {B}x{H}x{W} {Cin}->{Cout} k{k} res={res} obf16={obf} stats={stats} bn={bn}: {ms * 1e3:.1f} us  "
       f"{fl / ms / 1e9:.1f} TFLOP/s  {byts / ms / 1e6:.0f} GB/s (algorithmic bytes)")

@@ -27,7 +27,7 @@ with torch.no_grad():
 plan, _ = dec.plan_for(B, size, size)
 prof = plan.profile(reps=5)
 tot = sum(v["ms"] for v in prof.values())
-print(f"workload {wl} B={B} v2={plan.v2} bn_override={plan.bn_override}: sum of op times {tot:.2f} ms, {len(plan.ops)} ops")
+print(f"workload {wl} B={B} {prec}: sum of op times {tot:.2f} ms, {len(plan.ops)} ops")
 for k, v in sorted(prof.items(), key=lambda kv: -kv[1]["ms"]):
     tf = v["flops"] / (v["ms"] * 1e9) if v["flops"] else 0
     print(f"  {k:18s} {v['ms']:8.3f} ms  {100 * v['ms'] / tot:5.1f}%  n={v['launches']:4d}  {tf:8.1f} TFLOP/s")
@@ -37,17 +37,14 @@ for i, (fn, args) in enumerate(plan.ops):
         (s1, C1, s2, C2, sdt, ab, silu, w, bias, k1, S1, k2, S2, wsk, resid, out, odt, stats, Bb, H, W, Cout, bn) = args
         rows.append((plan.last_op_ms[i], f"conv_tc3 {H}x{W} {C1}+{C2}->{Cout} skip={S1 + S2} res={int(resid is not None)} obf16={odt}",
                      plan.flops[i]))
-    elif fn.startswith("conv_tc"):
+    elif fn.startswith("conv_tc2"):
         ints = [a for a in args if isinstance(a, int)]
         if fn == "conv_tc2_skip":
             odt, Bb, H, W, Cin, Cout, k, bn = ints[-8:]
             cv = 0
             fn = f"conv_tc2+skip{ints[0]}"
-        elif fn == "conv_tc2":
-            odt, Bb, H, W, Cin, Cout, k, cv, bn = ints[-9:]
         else:
-            Bb, H, W, Cin, Cout, k = ints[-6:]
-            odt = cv = 0
+            odt, Bb, H, W, Cin, Cout, k, cv, bn = ints[-9:]
         res = args[3] is not None
         rows.append((plan.last_op_ms[i], f"{fn} {H}x{W} {Cin}->{Cout} k{k} res={int(res)} obf16={odt} head={cv}", plan.flops[i]))
 agg = {}

@@ -10,12 +10,11 @@ from tests.util import assert_close
 pytestmark = pytest.mark.gpu
 
 
-def _run_conv(x, w, bias, resid, precision, k, out_dtype=torch.float32, want_stats=False, bn=0, v1=False):
+def _run_conv(x, w, bias, resid, precision, k, out_dtype=torch.float32, want_stats=False, bn=0):
     from pdae_b200.engine import Plan
     B, H, W, Cin = x.shape
     Cout = w.shape[0]
     P = Plan(x.device, precision)
-    P.v2 = not v1
     out = P.new((B, H, W, Cout), out_dtype)
     out.keep = True
     st = P.conv(P.fixed(x), w, bias, out, B=B, H=H, W=W, Cin=Cin, Cout=Cout, k=k,
@@ -59,12 +58,9 @@ def test_tc_conv_matches_simt(shape):
     resid = torch.randn(B, H, W, Cout, generator=g).cuda() if has_res else None
     y_tc, kinds = _run_conv(x, w, bias, resid, "bf16", k)
     assert kinds == ["conv_tc2"], kinds
-    y_v1, kinds = _run_conv(x, w, bias, resid, "bf16", k, v1=True)
-    assert kinds == ["conv_tc"], kinds
     y_ref, kinds = _run_conv(x, w, bias, resid, "fp32", k)
     assert kinds == ["conv2d_simt"], kinds
     assert_close(y_tc, y_ref, rtol=2e-3, atol=2e-3, what=f"tc v2 vs simt {shape}")
-    assert_close(y_v1, y_ref, rtol=2e-3, atol=2e-3, what=f"tc v1 vs simt {shape}")
     # every legal N tile of the persistent kernel
     for bn in (64, 128, 256):
         if Cout % bn == 0:

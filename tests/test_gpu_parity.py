@@ -147,8 +147,7 @@ def test_attention_tensor_core(C, heads, new_order):
     # split-operand mode: QK^T and PV as batched wgmma GEMMs on [hi|lo|hi] x [hi|hi|lo] operand blocks (fp32-grade)
     assert any(op[0] == "qkv_split3" for op in plan3.ops) and not any(op[0] == "attention_simt" for op in plan3.ops)
     plan = [v for k, v in m._plans().items() if k[1] == "bf16"][0][0]
-    if plan.v2:   # (the legacy v1 kernel, PDAE_TC_V1=1, has no batched-GEMM mode: CUDA-core attention there)
-        assert any(op[0].startswith("gemm_tc2") for op in plan.ops), "tensor-core attention path not taken"
+    assert any(op[0].startswith("gemm_tc2") for op in plan.ops), "tensor-core attention path not taken"
 
 
 @pytest.mark.parametrize("size,batch", [(24, 3), (48, 1), (40, 2)])
