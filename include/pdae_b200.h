@@ -207,6 +207,10 @@ typedef struct pdae_wgrad_tc_plan pdae_wgrad_tc_plan;
 int pdae_wgrad_tc_supported(int H, int W, int Cin, int Cout, int ksize);
 int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan, const void* act3_bf16, const void* dy3_bf16, float* dw, int B, int H, int W,
                          int Cin, int Cout, int ksize);
+/* Single-pass variant (bf16 autocast training): act / dy are plain bf16 NHWC tensors with Cin / Cout channels and every product
+ * is one bf16 MMA with fp32 accumulation.  Same shapes, zeroing contract and run / destroy functions as above. */
+int pdae_wgrad_tc_create_bf16(pdae_wgrad_tc_plan** plan, const void* act_bf16, const void* dy_bf16, float* dw, int B, int H, int W,
+                              int Cin, int Cout, int ksize);
 int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* plan, pdae_stream_t stream);
 void pdae_wgrad_tc_destroy(pdae_wgrad_tc_plan* plan);
 

@@ -107,6 +107,7 @@ _SIGS = {
     "pdae_conv_tc3_destroy": (None, [_P]),
     "pdae_wgrad_tc_supported": (c_int, [c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_create": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_wgrad_tc_create_bf16": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_run": (c_int, [_P, _P]),
     "pdae_wgrad_tc_destroy": (None, [_P]),
     "pdae_softmax_bf16": (c_int, [_P, _P, c_int64, c_int, c_float, _P]),

@@ -1,4 +1,5 @@
-// wgrad_tc -- weight gradient of a stride-1 3x3 / 1x1 "same" convolution on the tensor cores (sm_90a), fp32-grade.
+// wgrad_tc -- weight gradient of a stride-1 3x3 / 1x1 "same" convolution on the tensor cores (sm_90a): fp32-grade on split
+// operands, or single-pass on plain bf16 operands (the bf16 autocast training step).
 //
 //   dW[tap][cin][cout] = sum over (b, y, x) of  act[b, y+dy, x+dx, cin] * dY[b, y, x, cout]        (autograd of F.conv2d,
 //   model/module.py:241-243, 255-259 under trainer/train_representation_learning.py:112 loss.backward())
@@ -9,8 +10,10 @@
 // further supplies channels 64-127.  One k-step = 128 (M channels) x BN (N channels) x 16 pixels, as two m64 wgmmas (one per
 // consumer warpgroup).
 //
-// Operands arrive split, [hi | lo | hi] channel blocks (a = hi + lo, bf16 each): every product is
+// SPLIT = true: operands arrive split, [hi | lo | hi] channel blocks (a = hi + lo, bf16 each): every product is
 // a_hi*d_hi + a_lo*d_hi + a_hi*d_lo accumulated in fp32 registers -- the same fp32-grade scheme as the forward / dgrad convs.
+// SPLIT = false: operands are plain bf16 tensors with C channels; a stage holds one block per operand and a k-step issues one
+// wgmma per warpgroup (a third of the MMA work and of the operand bytes), still accumulated in fp32.
 //
 // Work item = (tap, M chunk of 128 channels, N chunk of BN channels, 64-pixel tile).  Items are dealt to the persistent CTAs
 // in contiguous ranges (split-K over pixels); a CTA accumulates in registers while consecutive items belong to the same
@@ -32,13 +35,15 @@ namespace pdae {
 constexpr int WG_KT = 64;                 // pixels per k-tile (= rows of one TMA box)
 constexpr int WG_BOX = WG_KT * 128;       // bytes of one [64 px][64 ch] box
 constexpr int WG_THREADS = 288;
-constexpr int WG_MAX_ST = 4;
+constexpr int WG_MAX_ST = 4;              // stage ring depth cap of the split variant (its 48-64 KB stages fit 3-4)
+constexpr int WG_MAX_ST_BF16 = 8;         // plain bf16 variant: 24-32 KB stages, up to 8 in the same shared-memory budget
+constexpr int WG_SMEM_BUDGET = 220 * 1024;
 
 struct WgradArgs {
   float* dw;
   long long sm, sn, stap;   // element strides of the (m, n, tap) indices inside dw
   int a_is_act;             // 1: M side = activation (shifted per tap), N side = dY; 0: M side = dY, N side = activation
-  int Ma, Nb;               // real channel counts on the M / N side (the tensors hold 3x: [hi | lo | hi])
+  int Ma, Nb;               // real channel counts on the M / N side (split operands hold 3x: [hi | lo | hi])
   int mchunks, nchunks, taps, ksize;
   int pair;                 // 1: 64-channel M chunks, the 128 accumulator rows hold TWO taps (activation on the M side)
   int tw, th, tn, tiles_x, tiles_y, tiles_b, ktiles;
@@ -87,16 +92,18 @@ __device__ __forceinline__ bool elect_one() {
 }
 }  // namespace wg
 
-template <int BN>
+template <int BN, bool SPLIT>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, WgradArgs p) {
   using namespace wg;
   extern __shared__ uint8_t smem_raw[];
-  __shared__ __align__(8) uint64_t bar_full[WG_MAX_ST], bar_empty[WG_MAX_ST];
+  constexpr int MAX_ST = SPLIT ? WG_MAX_ST : WG_MAX_ST_BF16;
+  __shared__ __align__(8) uint64_t bar_full[MAX_ST], bar_empty[MAX_ST];
   constexpr int NBOX_B = BN / 64;                       // 64-channel boxes of the N-side tile
   constexpr int A_BYTES = 2 * WG_BOX;                   // M = 128 channels = two boxes
   constexpr int B_BYTES = NBOX_B * WG_BOX;
-  constexpr int STAGE = 2 * A_BYTES + 2 * B_BYTES;      // (hi, lo) of both operands
+  constexpr int NBLK = SPLIT ? 2 : 1;                   // channel blocks loaded per operand: (hi, lo) or the plain tensor
+  constexpr int STAGE = NBLK * (A_BYTES + B_BYTES);
   const uint32_t smem0 = (s_u32(smem_raw) + 1023u) & ~1023u;
   const int S = p.stages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -150,13 +157,13 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       if (elect_one()) {
         mb_expect_tx(full, (uint32_t)STAGE);
 #pragma unroll
-        for (int h = 0; h < 2; ++h) {          // hi block (channel offset 0), lo block (channel offset Ma / Nb)
+        for (int h = 0; h < NBLK; ++h) {       // hi block (channel offset 0), lo block (channel offset Ma / Nb)
 #pragma unroll
           for (int j = 0; j < 2; ++j)
             tma_ld4(base + (uint32_t)(h * A_BYTES + j * WG_BOX), &tmA, full, h * p.Ma + am[j], ax[j], ay[j], b0);
 #pragma unroll
           for (int j = 0; j < NBOX_B; ++j)
-            tma_ld4(base + (uint32_t)(2 * A_BYTES + h * B_BYTES + j * WG_BOX), &tmB, full, h * p.Nb + n0 + j * 64, bx, by, b0);
+            tma_ld4(base + (uint32_t)(NBLK * A_BYTES + h * B_BYTES + j * WG_BOX), &tmB, full, h * p.Nb + n0 + j * 64, bx, by, b0);
         }
       }
       __syncwarp();
@@ -196,16 +203,27 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
       mb_wait(s_u32(&bar_full[s]), ph);
       const uint32_t base = smem0 + (uint32_t)(s * STAGE) + (uint32_t)(wgi * WG_BOX);
-      const uint64_t a_hi = wgmma::desc_sw128(base, WG_BOX, 1024u), a_lo = wgmma::desc_sw128(base + A_BYTES, WG_BOX, 1024u);
-      const uint32_t bb = smem0 + (uint32_t)(s * STAGE) + 2u * A_BYTES;
-      const uint64_t b_hi = wgmma::desc_sw128(bb, WG_BOX, 1024u), b_lo = wgmma::desc_sw128(bb + B_BYTES, WG_BOX, 1024u);
-      wgmma::fence();
+      if constexpr (SPLIT) {
+        const uint64_t a_hi = wgmma::desc_sw128(base, WG_BOX, 1024u), a_lo = wgmma::desc_sw128(base + A_BYTES, WG_BOX, 1024u);
+        const uint32_t bb = smem0 + (uint32_t)(s * STAGE) + 2u * A_BYTES;
+        const uint64_t b_hi = wgmma::desc_sw128(bb, WG_BOX, 1024u), b_lo = wgmma::desc_sw128(bb + B_BYTES, WG_BOX, 1024u);
+        wgmma::fence();
 #pragma unroll
-      for (int k = 0; k < WG_KT / 16; ++k) {           // 16 pixels per k-step = 16 rows x 128 B = 2048 B = 128 descriptor units
-        const uint64_t o = (uint64_t)(k * 128);
-        wgmma::mma<BN, 1>(acc, a_hi + o, b_hi + o, (uint32_t)(!(first && k == 0)));
-        wgmma::mma<BN, 1>(acc, a_lo + o, b_hi + o, 1u);
-        wgmma::mma<BN, 1>(acc, a_hi + o, b_lo + o, 1u);
+        for (int k = 0; k < WG_KT / 16; ++k) {         // 16 pixels per k-step = 16 rows x 128 B = 2048 B = 128 descriptor units
+          const uint64_t o = (uint64_t)(k * 128);
+          wgmma::mma<BN, 1>(acc, a_hi + o, b_hi + o, (uint32_t)(!(first && k == 0)));
+          wgmma::mma<BN, 1>(acc, a_lo + o, b_hi + o, 1u);
+          wgmma::mma<BN, 1>(acc, a_hi + o, b_lo + o, 1u);
+        }
+      } else {                                          // plain bf16: one wgmma per k-step
+        const uint64_t a_d = wgmma::desc_sw128(base, WG_BOX, 1024u);
+        const uint64_t b_d = wgmma::desc_sw128(smem0 + (uint32_t)(s * STAGE) + (uint32_t)A_BYTES, WG_BOX, 1024u);
+        wgmma::fence();
+#pragma unroll
+        for (int k = 0; k < WG_KT / 16; ++k) {
+          const uint64_t o = (uint64_t)(k * 128);
+          wgmma::mma<BN, 1>(acc, a_d + o, b_d + o, (uint32_t)(!(first && k == 0)));
+        }
       }
       wgmma::commit();
       wgmma::wait<0>();
@@ -239,15 +257,15 @@ static int pow2_tile_w(int W, int cap) {
   return t;
 }
 
-template <int BN>
+template <int BN, bool SPLIT>
 static cudaError_t launch_wg(const CUtensorMap& a, const CUtensorMap& b, const WgradArgs& args, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<BN>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<BN, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  wgrad_tc_kernel<BN><<<grid, WG_THREADS, smem, s>>>(a, b, args);
+  wgrad_tc_kernel<BN, SPLIT><<<grid, WG_THREADS, smem, s>>>(a, b, args);
   return cudaPeekAtLastError();
 }
 
@@ -258,7 +276,7 @@ using namespace pdae;
 struct pdae_wgrad_tc_plan {
   CUtensorMap tmA, tmB;
   WgradArgs args;
-  int BN, grid;
+  int BN, split, grid;
   size_t smem;
 };
 
@@ -272,13 +290,14 @@ extern "C" int pdae_wgrad_tc_supported(int H, int W, int Cin, int Cout, int ksiz
   return (W % tw == 0 && H % th == 0 && tw * th * tn == WG_KT && tn <= 64) ? 1 : 0;
 }
 
-extern "C" int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan_out, const void* act3_bf16, const void* dy3_bf16, float* dw, int B,
-                                    int H, int W, int Cin, int Cout, int ksize) {
-  PDAE_REQUIRE(plan_out && act3_bf16 && dy3_bf16 && dw, "wgrad_tc_create: null pointer");
+// split: act / dy hold [hi | lo | hi] blocks of 3*C channels; otherwise plain bf16 with C channels
+static int wgrad_create(pdae_wgrad_tc_plan** plan_out, const void* act, const void* dy, float* dw, int B, int H, int W, int Cin,
+                        int Cout, int ksize, bool split) {
+  PDAE_REQUIRE(plan_out && act && dy && dw, "wgrad_tc_create: null pointer");
   PDAE_REQUIRE(pdae_wgrad_tc_supported(H, W, Cin, Cout, ksize), "wgrad_tc_create: unsupported shape H=%d W=%d Cin=%d Cout=%d k=%d", H, W,
                Cin, Cout, ksize);
-  PDAE_REQUIRE(!(((uintptr_t)act3_bf16 | (uintptr_t)dy3_bf16) & 15) && !((uintptr_t)dw & 3),
-               "wgrad_tc_create: act3 / dy3 must be 16-byte aligned (TMA), dw 4-byte aligned");
+  PDAE_REQUIRE(!(((uintptr_t)act | (uintptr_t)dy) & 15) && !((uintptr_t)dw & 3),
+               "wgrad_tc_create: act / dy must be 16-byte aligned (TMA), dw 4-byte aligned");
   EncodeTiledFnW enc = encode_fnw();
   PDAE_REQUIRE(enc != nullptr, "wgrad_tc_create: cuTensorMapEncodeTiled unavailable (no driver)");
   if (g_num_sms_w == 0) {
@@ -298,21 +317,23 @@ extern "C" int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan_out, const void* a
   a.stap = (long long)Cin * Cout;
   const int BN = (a.Nb % 128 == 0) ? 128 : 64;
   pl->BN = BN;
+  pl->split = split ? 1 : 0;
   a.mchunks = a.pair ? a.Ma / 64 : a.Ma / 128; a.nchunks = a.Nb / BN; a.taps = ksize * ksize; a.ksize = ksize;
   a.tw = pow2_tile_w(W, WG_KT); a.th = pow2_tile_w(H, WG_KT / a.tw); a.tn = WG_KT / (a.tw * a.th);
   a.tiles_x = W / a.tw; a.tiles_y = H / a.th; a.tiles_b = (B + a.tn - 1) / a.tn;
   a.ktiles = a.tiles_x * a.tiles_y * a.tiles_b;
   a.B = B; a.H = H; a.W = W;
   a.items = (long long)(a.pair ? (a.taps + 1) / 2 : a.taps) * a.mchunks * a.nchunks * a.ktiles;
-  const int stage = 2 * (2 * WG_BOX) + 2 * (BN / 64) * WG_BOX;
-  int stages = (220 * 1024 - 1024) / stage;
-  if (stages > WG_MAX_ST) stages = WG_MAX_ST;
+  const int stage = (split ? 2 : 1) * (2 * WG_BOX + (BN / 64) * WG_BOX);
+  const int max_st = split ? WG_MAX_ST : WG_MAX_ST_BF16;
+  int stages = (WG_SMEM_BUDGET - 1024) / stage;
+  if (stages > max_st) stages = max_st;
   a.stages = stages;
   pl->smem = (size_t)stages * stage + 1024;
   pl->grid = a.items < g_num_sms_w ? (int)a.items : g_num_sms_w;
-  const void* At = a.a_is_act ? act3_bf16 : dy3_bf16;
-  const void* Bt = a.a_is_act ? dy3_bf16 : act3_bf16;
-  const int Ca = 3 * a.Ma, Cb = 3 * a.Nb;
+  const void* At = a.a_is_act ? act : dy;
+  const void* Bt = a.a_is_act ? dy : act;
+  const int Ca = (split ? 3 : 1) * a.Ma, Cb = (split ? 3 : 1) * a.Nb;
   cuuint32_t estr4[4] = {1, 1, 1, 1};
   cuuint32_t box[4] = {64, (cuuint32_t)a.tw, (cuuint32_t)a.th, (cuuint32_t)a.tn};
   for (int i = 0; i < 2; ++i) {
@@ -332,14 +353,29 @@ extern "C" int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan_out, const void* a
   return PDAE_OK;
 }
 
+extern "C" int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan_out, const void* act3_bf16, const void* dy3_bf16, float* dw, int B,
+                                    int H, int W, int Cin, int Cout, int ksize) {
+  return wgrad_create(plan_out, act3_bf16, dy3_bf16, dw, B, H, W, Cin, Cout, ksize, true);
+}
+
+extern "C" int pdae_wgrad_tc_create_bf16(pdae_wgrad_tc_plan** plan_out, const void* act_bf16, const void* dy_bf16, float* dw, int B,
+                                         int H, int W, int Cin, int Cout, int ksize) {
+  return wgrad_create(plan_out, act_bf16, dy_bf16, dw, B, H, W, Cin, Cout, ksize, false);
+}
+
 extern "C" int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* pl, pdae_stream_t stream) {
   PDAE_REQUIRE(pl, "wgrad_tc_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
-  cudaError_t e = pl->BN == 128 ? launch_wg<128>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s)
-                                : launch_wg<64>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s);
+  cudaError_t e;
+  if (pl->split)
+    e = pl->BN == 128 ? launch_wg<128, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s)
+                      : launch_wg<64, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s);
+  else
+    e = pl->BN == 128 ? launch_wg<128, false>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s)
+                      : launch_wg<64, false>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s);
   if (e != cudaSuccess) {
     (void)cudaGetLastError();
-    set_error("launch of wgrad_tc_kernel<%d> failed: %s", pl->BN, cudaGetErrorString(e));
+    set_error("launch of wgrad_tc_kernel<%d, %s> failed: %s", pl->BN, pl->split ? "split" : "bf16", cudaGetErrorString(e));
     return PDAE_ECUDA;
   }
   return PDAE_OK;

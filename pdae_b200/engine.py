@@ -50,7 +50,7 @@ def get_default_precision() -> str:
 
 class Buf:
     """A device buffer known to a plan: either plan-owned (arena) or fixed (parameter / caller tensor)."""
-    __slots__ = ("shape", "dtype", "tensor", "first", "last", "fixed", "keep", "name", "_block", "split3", "split3_copy")
+    __slots__ = ("shape", "dtype", "tensor", "first", "last", "fixed", "keep", "name", "_block", "split3", "tc_copy")
 
     def __init__(self, shape, dtype, tensor=None, name=""):
         self.shape = tuple(int(s) for s in shape)
@@ -62,7 +62,7 @@ class Buf:
         self.keep = False
         self.name = name
         self.split3 = False   # "bf16x3" activation: last dim holds three bf16 channel blocks [hi | lo | hi]
-        self.split3_copy = None   # training forward: the [hi | lo | hi] copy of this fp32 activation (Plan.conv, train_tc)
+        self.tc_copy = None   # training forward: the bf16 tensor-core copy of this fp32 activation (Plan.conv, train_tc)
 
     @property
     def nbytes(self) -> int:
@@ -153,9 +153,10 @@ class Plan:
         self._nplan_handles: List[ctypes.c_void_p] = []
         self._native_plans: dict = {}
         self.head_fuse: Dict[str, Buf] = {}   # image heads whose epilogue can run the DDIM update (set by a sampling loop)
-        # training forward plans (fp32, every intermediate kept for the backward): run the eligible convs on the tensor cores in
-        # the split-operand mode -- the fp32 activation the backward needs stays as it is, a [hi | lo | hi] copy feeds conv_tc2
-        self.train_tc = False
+        # training forward plans (fp32, every intermediate kept for the backward): the precision of the eligible convs on the
+        # tensor cores.  None: CUDA cores; "bf16x3": split operands (a [hi | lo | hi] copy of the fp32 activation feeds conv_tc2);
+        # "bf16": a plain bf16 copy feeds conv_tc2 (autocast training).  The fp32 activation the backward needs stays as it is.
+        self.train_tc: Optional[str] = None
         self.n_launch = 0
         self.keep_all = False
         self.dropout_masks: list = []   # (block, mask buffer, p): filled by the trainer before every training forward
@@ -307,8 +308,8 @@ class Plan:
             if fn == "conv_tc3":
                 compiled.append(self._compile_tc3(args))
                 continue
-            if fn == "wgrad_tc":
-                compiled.append(self._compile_wgrad(args))
+            if fn in ("wgrad_tc", "wgrad_tc_bf16"):
+                compiled.append(self._compile_wgrad(args, split=fn == "wgrad_tc"))
                 continue
             cargs = []
             sidx = -1
@@ -383,14 +384,14 @@ class Plan:
         self._tc3_handles.append(h)
         return (self.L.pdae_conv_tc3_run, [h, None], 1, "conv_tc3")
 
-    def _compile_wgrad(self, args):
-        act3, dy3, dw, B, H, W, Cin, Cout, k = args
+    def _compile_wgrad(self, args, split: bool):
+        act, dy, dw, B, H, W, Cin, Cout, k = args
         h = ctypes.c_void_p()
-        rc = self.L.pdae_wgrad_tc_create(ctypes.byref(h), self._resolve(act3), self._resolve(dy3), self._resolve(dw), B, H, W, Cin,
-                                         Cout, k)
-        _native.check(rc, "pdae_wgrad_tc_create")
+        create = self.L.pdae_wgrad_tc_create if split else self.L.pdae_wgrad_tc_create_bf16
+        rc = create(ctypes.byref(h), self._resolve(act), self._resolve(dy), self._resolve(dw), B, H, W, Cin, Cout, k)
+        _native.check(rc, create.__name__)
         self._wg_handles.append(h)
-        return (self.L.pdae_wgrad_tc_run, [h, None], 1, "wgrad_tc")
+        return (self.L.pdae_wgrad_tc_run, [h, None], 1, "wgrad_tc" if split else "wgrad_tc_bf16")
 
     def _compile_gemm_softmax(self, args):
         a, a_ld, a_bs, b, b_ld, b_bs, out, o_ld, o_bs, batch, M, N, K, alpha = args
@@ -566,13 +567,24 @@ class Plan:
         pad = k // 2 if pad is None else pad
         if (self.train_tc and x.dtype == torch.float32 and out.dtype == torch.float32 and not (in_nchw or out_nchw or a_silu)
                 and skip is None and w_transform is None and pad == k // 2 and self._tc_shape_ok(Cin, Cout, k, stride, H, W)):
-            x3b = self.new((B, H, W, 3 * Cin), torch.bfloat16, "train_split3")
-            x3b.split3 = True
-            x.split3_copy = x3b      # the backward's tensor-core weight gradient reads the same split activation
-            self.call("gn_apply_split3", x, Cin, None, 0, None, 0, RESAMPLE_NONE, B, H, W, x3b, None, PDAE_F32, _STREAM)
-            wp = self.pack((wkey or id(weight), "tc_x3"), [weight],
-                           lambda Cin=Cin: split3_weights(weight.detach().reshape(Cout, Cin, k * k)))
-            self.call("conv_tc2", x3b, wp, self.param(bias), residual, out, PDAE_F32, None, B, H, W, 3 * Cin, Cout, k, 0,
+            if self.train_tc == "bf16x3":
+                xt = self.new((B, H, W, 3 * Cin), torch.bfloat16, "train_split3")
+                xt.split3 = True
+                self.call("gn_apply_split3", x, Cin, None, 0, None, 0, RESAMPLE_NONE, B, H, W, xt, None, PDAE_F32, _STREAM)
+                wp = self.pack((wkey or id(weight), "tc_x3"), [weight],
+                               lambda Cin=Cin: split3_weights(weight.detach().reshape(Cout, Cin, k * k)))
+                Ce = 3 * Cin
+            elif self.train_tc == "bf16":
+                xt = self.new((B, H, W, Cin), torch.bfloat16, "train_bf16")
+                self.call("gn_apply", x, PDAE_F32, Cin, None, PDAE_F32, 0, None, 0, RESAMPLE_NONE, B, H, W, xt, PDAE_BF16, None,
+                          PDAE_F32, _STREAM)
+                wp = self.pack((wkey or id(weight), "tc"), [weight],
+                               lambda: weight.detach().reshape(Cout, Cin, k * k).permute(2, 0, 1).to(torch.bfloat16))
+                Ce = Cin
+            else:
+                raise ValueError(f"Plan.train_tc must be None, 'bf16x3' or 'bf16', not {self.train_tc!r}")
+            x.tc_copy = xt      # the backward's tensor-core weight gradient reads the same bf16 activation
+            self.call("conv_tc2", xt, wp, self.param(bias), residual, out, PDAE_F32, None, B, H, W, Ce, Cout, k, 0,
                       bn_override, flops=2.0 * B * H * W * Cout * Cin * k * k)
             return None
         bias_b = self.param(bias)

@@ -11,6 +11,12 @@ split operands (``Plan.train_tc``, ``bwd_plan``, ``pdae_wgrad_tc_*``).  GroupNor
 stride-2 / 3-channel convs stay fp32 on CUDA cores (``pdae_gn_bwd_*``, ``pdae_gemm_batched_simt``, ``pdae_softmax_bwd``,
 ``pdae_conv2d_wgrad_simt`` / ``pdae_conv2d_dgrad_simt``).  Gradients reach autograd through one ``pdae_unpack_grads`` launch
 (``GradSink``).  Dropout is inverted dropout with masks drawn by torch's CUDA generator.
+
+Mixed precision: a ShiftUNet / UNet training forward called inside ``torch.autocast("cuda")`` (the reference trainers'
+``enable_amp``; either autocast dtype) builds separate bf16 trainers: the frozen half runs as a plain "bf16" plan, and the
+forward convs, data gradients and weight gradients of the trainable convs are single-pass bf16 MMAs with fp32 accumulation.
+Activations, GroupNorm, attention and every gradient stay fp32, so the reference's ``GradScaler`` works unchanged.  The
+encoder and the latent MLP ignore autocast.
 """
 from __future__ import annotations
 
@@ -101,11 +107,17 @@ def draw_dropout_masks(plan: Plan) -> None:
         mask.tensor.bernoulli_(1.0 - p)
 
 
-def bwd_plan(dev) -> Plan:
-    """Backward plans are split-operand tensor-core plans: the data gradient of every eligible stride-1 conv runs on
-    `conv_tc2` and its weight gradient on `wgrad_tc`, both in the fp32-grade "bf16x3" mode (Backward.conv); everything else
-    in them is fp32 CUDA-core arithmetic."""
-    return Plan(dev, "bf16x3")
+def bwd_plan(dev, amp: bool = False) -> Plan:
+    """Backward plans are tensor-core plans: the data gradient of every eligible stride-1 conv runs on `conv_tc2` and its
+    weight gradient on `wgrad_tc`, both in the fp32-grade split-operand "bf16x3" mode, or with `amp` in the single-pass
+    "bf16" mode (Backward.conv); everything else in them is fp32 CUDA-core arithmetic."""
+    return Plan(dev, "bf16" if amp else "bf16x3")
+
+
+def autocast_active() -> bool:
+    """Is the caller inside an enabled CUDA autocast region?  Either autocast dtype selects the bf16 training plans: there
+    are no fp16 kernels, and bf16 has fp32's exponent range, so a GradScaler's scale never overflows them."""
+    return torch.is_autocast_enabled("cuda")
 
 
 class Backward:
@@ -137,20 +149,23 @@ class Backward:
         Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
         kk = k * k
         same = stride == 1 and k in (1, 3) and pad == k // 2 and not in_nchw
+        # tensor-core operands: split [hi | lo | hi] blocks in the "bf16x3" backward, plain bf16 in the "bf16" (autocast) one
+        ce = 3 if P.x3 else 1
         dy3 = None
         if trainable:
             dw = P.new_zeroed(kk * Cin * Cout)
             if same and not a_silu and P.L.pdae_wgrad_tc_supported(H, W, Cin, Cout, k):
-                # weight gradient on the tensor cores (wgrad_tc.cu): both operands split [hi | lo | hi], fp32-grade products
-                a3 = getattr(x, "split3_copy", None)       # left by the tensor-core training forward (Plan.conv, train_tc)
-                if a3 is not None and tuple(a3.shape) == (B, H, W, 3 * Cin):
+                # weight gradient on the tensor cores (wgrad_tc.cu): fp32-grade split products, or single-pass bf16
+                a3 = getattr(x, "tc_copy", None)       # left by the tensor-core training forward (Plan.conv, train_tc)
+                if a3 is not None and tuple(a3.shape) == (B, H, W, ce * Cin):
                     a3 = self.fx(a3)
                 else:
                     a3, _ = P.gn_apply(self.fx(x), Cin, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=H, W=W,
                                        act_dtype=torch.bfloat16)
                 dy3, _ = P.gn_apply(dy, Cout, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=H, W=W,
                                     act_dtype=torch.bfloat16)
-                P.call("wgrad_tc", a3, dy3, dw, B, H, W, Cin, Cout, k, flops=2.0 * B * H * W * Cin * Cout * kk)
+                P.call("wgrad_tc" if P.x3 else "wgrad_tc_bf16", a3, dy3, dw, B, H, W, Cin, Cout, k,
+                       flops=2.0 * B * H * W * Cin * Cout * kk)
             else:
                 P.call("conv2d_wgrad_simt", self.fx(x), int(in_nchw), int(a_silu), dy, dw, B, H, W, Cin, Cout, k, stride, pad,
                        _STREAM)
@@ -164,7 +179,8 @@ class Backward:
             return None
         if same and P.use_tc(Cout, Cin, k, 1, H, W):
             # dgrad of a stride-1 "same" conv = conv of dy with the transposed, spatially flipped weights: on the tensor
-            # cores in the split-operand (fp32-grade) mode -- dy is split [hi | lo | hi], W' packed [W'_hi | W'_hi | W'_lo]
+            # cores in the split-operand (fp32-grade) mode -- dy is split [hi | lo | hi], W' packed [W'_hi | W'_hi | W'_lo] --
+            # or, in the "bf16" backward, as one bf16 product of plain dy and W' ("tc" pack)
             if dy3 is None:
                 dy3, _ = P.gn_apply(dy, Cout, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=H, W=W,
                                     act_dtype=torch.bfloat16)
@@ -323,9 +339,10 @@ class _Generation:
 
 
 class ShiftUNetTrainer(_Generation):
-    """Forward (fp32, all intermediates kept) + backward plans of a ShiftUNet for one input shape."""
+    """Forward (fp32, all intermediates kept) + backward plans of a ShiftUNet for one input shape; `amp`: the bf16 plans of
+    a forward under autocast (module docstring)."""
 
-    def __init__(self, net, B: int, H: int, W: int):
+    def __init__(self, net, B: int, H: int, W: int, amp: bool = False):
         from .model.unet import EmbBank, emit_head, emit_stem, emit_time_embed, res_blocks_of
         self.net = net
         dev = net._device()
@@ -334,9 +351,10 @@ class ShiftUNetTrainer(_Generation):
         frozen_blocks = res_blocks_of(net.input_blocks, net.middle_block, net.output_blocks)
         # The FROZEN half (input / middle / output blocks, `out` head: 55 % of the forward FLOPs) builds no autograd graph in
         # the reference either (its parameters do not require grad): it runs as a tensor-core plan in the split-operand
-        # (fp32-grade) mode with the fused-prologue convs, exactly like sampling; only its skip tensors and bottleneck output
-        # are handed to the trainable half.
-        Fp = Plan(dev, "bf16x3")
+        # (fp32-grade) mode -- or, with amp, in the plain "bf16" mode -- with the fused-prologue convs, exactly like sampling;
+        # only its skip tensors and bottleneck output are handed to the trainable half.
+        self.amp = amp
+        Fp = Plan(dev, "bf16" if amp else "bf16x3")
         self.x_in = Fp.new((B, net.input_channel, H, W), torch.float32, "x_nchw")
         self.t_in = Fp.new((B,), torch.int64, "t")
         self.x_in.keep = self.t_in.keep = True
@@ -347,8 +365,14 @@ class ShiftUNetTrainer(_Generation):
         for stage in list(net.input_blocks)[1:]:
             hf = stage.emit(Fp, hf, bank_f)
             hs_f.append(hf)
-        for sfrc in hs_f:                      # consumed by the trainable half's plan: private storage
-            sfrc.b1.keep = True
+        skips = []                             # consumed by the trainable half's plan: private storage
+        for sfrc in hs_f:
+            b = sfrc.b1
+            if b.dtype != torch.float32:       # bf16 residual stream (amp): widened to fp32 once per step
+                b, _ = Fp.gn_apply(b, sfrc.C, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=sfrc.H, W=sfrc.W,
+                                   act_dtype=torch.float32)
+            b.keep = True
+            skips.append((b, sfrc))
         eps_h = net.middle_block.emit(Fp, hf, bank_f)
         for stage, skip in zip(net.output_blocks, reversed(hs_f)):
             eps_h = stage.emit(Fp, eps_h.cat(skip), bank_f)
@@ -359,7 +383,7 @@ class ShiftUNetTrainer(_Generation):
         self.frozen = Fp
         P = Plan(dev, "fp32")
         P.keep_all = True
-        P.train_tc = True         # trainable half: fp32 activations kept for the backward, convs on the tensor cores (split operands)
+        P.train_tc = "bf16" if amp else "bf16x3"   # trainable half: fp32 activations kept, convs on the tensor cores
         self.z_in = P.new((B, net.latent_dim), torch.float32, "z")
         emb = emit_time_embed(P, net.time_embed, P.fixed(self.t_in.tensor), B, base, E, dev)
         shift_emb = P.new((B, E), torch.float32, "shift_emb")
@@ -367,7 +391,7 @@ class ShiftUNetTrainer(_Generation):
         bank_t = EmbBank(P, shift_blocks, "t", emb, B, E, "train_t_shift")
         bank_z = EmbBank(P, shift_blocks, "z", shift_emb, B, E, "train_z_shift")
         tape: list = []
-        hs = [Src(P.fixed(sfrc.b1.tensor), sfrc.C, B, sfrc.H, sfrc.W) for sfrc in hs_f]
+        hs = [Src(P.fixed(b.tensor), sfrc.C, B, sfrc.H, sfrc.W) for b, sfrc in skips]
         shift_h = net.shift_middle_block.emit(P, hs[-1], bank_t, bank_z, tape=tape)
         for shift_stage in net.shift_output_blocks:
             shift_h = shift_stage.emit(P, shift_h.cat(hs.pop()), bank_t, bank_z, tape=tape)
@@ -377,7 +401,7 @@ class ShiftUNetTrainer(_Generation):
         self.fwd = P
 
         # ---------------- backward plan ----------------
-        BP = bwd_plan(dev)
+        BP = bwd_plan(dev, amp)
         self.sink = GradSink()
         bw = Backward(BP, self.sink)
         self.d_grad = BP.new((B, net.input_channel, H, W), torch.float32, "d_shift_nchw")
@@ -447,11 +471,12 @@ class _ShiftUNetFn(torch.autograd.Function):
 
 def shiftunet_train_forward(net, x, t, z):
     B, C, H, W = x.shape
-    key = ("train", B, H, W, tuple(m.training for m in net._shift_parts()))
+    amp = autocast_active()
+    key = ("train", B, H, W, tuple(m.training for m in net._shift_parts()), amp)
     cache = net.__dict__.setdefault("_train_cache", {})
     tr = cache.get(key)
     if tr is None or tr.stale():
-        tr = ShiftUNetTrainer(net, B, H, W)
+        tr = ShiftUNetTrainer(net, B, H, W, amp)
         cache[key] = tr
     return _ShiftUNetFn.apply(tr, x, t, z, *tr.params)
 
@@ -460,14 +485,15 @@ def shiftunet_train_forward(net, x, t, z):
 # Plain UNet (regular DPM training, gaussian_diffusion.py:199-211) -- every parameter trainable, skip gradients routed
 # ======================================================================================================================
 class UNetTrainer(_Generation):
-    def __init__(self, net, B: int, H: int, W: int):
+    def __init__(self, net, B: int, H: int, W: int, amp: bool = False):
         from .model.unet import EmbBank, emit_head, res_blocks_of
         from .model.module import timestep_freqs
         self.net = net
+        self.amp = amp
         dev = net._device()
         P = Plan(dev, "fp32")
         P.keep_all = True
-        P.train_tc = True         # convs on the tensor cores (split operands), fp32 activations kept
+        P.train_tc = "bf16" if amp else "bf16x3"   # convs on the tensor cores, fp32 activations kept
         E, base, Cimg = net.time_embed_dim, net.base_channel, net.input_channel
         self.x_in = P.new((B, Cimg, H, W), torch.float32, "x_nchw")
         self.t_in = P.new((B,), torch.int64, "t")
@@ -509,7 +535,7 @@ class UNetTrainer(_Generation):
         P.finalize()
         self.fwd = P
 
-        BP = bwd_plan(dev)
+        BP = bwd_plan(dev, amp)
         self.sink = GradSink()
         bw = Backward(BP, self.sink)
         self.d_out = BP.new((B, net.output_channel, H, W), torch.float32, "d_eps_nchw")
@@ -594,10 +620,11 @@ class _UNetFn(torch.autograd.Function):
 def unet_train_forward(net, x, t, cond):
     B, C, H, W = x.shape
     cache = net.__dict__.setdefault("_train_cache", {})
-    key = (B, H, W, net.training)
+    amp = autocast_active()
+    key = (B, H, W, net.training, amp)
     tr = cache.get(key)
     if tr is None or tr.fwd.stale() or tr.bwd.stale():
-        tr = UNetTrainer(net, B, H, W)
+        tr = UNetTrainer(net, B, H, W, amp)
         cache[key] = tr
     return _UNetFn.apply(tr, x, t, cond, *tr.params)
 

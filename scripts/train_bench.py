@@ -1,11 +1,13 @@
 """Training-step throughput (SURVEY.md section 8(d) config 5): representation_learning_train_one_batch + backward + gradient
 all-reduce + fused Adam/EMA step on the celeba64-proxy decoder + encoder.
 
-  python scripts/train_bench.py [--batch 32] [--steps 5]                                   # 1 GPU
+  python scripts/train_bench.py [--batch 32] [--steps 5] [--amp {off,bf16}]               # 1 GPU
   python -m torch.distributed.run --nproc-per-node N ... scripts/train_bench.py --overlap 1   # N GPUs, batch per GPU fixed
 
 Arithmetic: decoder forward, data gradients (conv_tc2) and weight gradients (wgrad_tc) on the tensor cores in the
-split-operand fp32-grade mode; encoder and the stride-2 / 3-channel convs in fp32 on CUDA cores (DESIGN.md).  --overlap 1: the decoder bucket's NCCL all-reduce is launched from a
+split-operand fp32-grade mode; encoder and the stride-2 / 3-channel convs in fp32 on CUDA cores (DESIGN.md).  --amp bf16: the step
+runs inside torch.autocast("cuda", dtype=torch.bfloat16) (the reference's enable_amp), so the decoder trains on the bf16
+plans: frozen half in the "bf16" mode, single-pass bf16 forward convs, data and weight gradients.  --overlap 1: the decoder bucket's NCCL all-reduce is launched from a
 post-accumulate-grad hook as soon as the ShiftUNet backward has delivered its gradients and runs while the encoder
 backward computes (pdae_b200.utils.dist.OverlappedGradAllReduce); --overlap 0: all-reduce after backward.
 Rank 0 prints one JSON line."""
@@ -31,6 +33,7 @@ ap = argparse.ArgumentParser()
 ap.add_argument("--batch", type=int, default=32)
 ap.add_argument("--steps", type=int, default=5)
 ap.add_argument("--overlap", type=int, default=1)
+ap.add_argument("--amp", choices=("off", "bf16"), default="off")
 args = ap.parse_args()
 world = int(os.environ.get("WORLD_SIZE", "1"))
 rank = int(os.environ.get("RANK", "0"))
@@ -62,7 +65,8 @@ all_params = [p for g in groups for p in g]
 
 
 def step():
-    loss = gd.representation_learning_train_one_batch(enc, dec, x0)["prediction_loss"]
+    with torch.autocast("cuda", dtype=torch.bfloat16, enabled=args.amp == "bf16"):
+        loss = gd.representation_learning_train_one_batch(enc, dec, x0)["prediction_loss"]
     loss.backward()
     scale = red.finish() if red is not None else allreduce_grads_(all_params)
     opt.step(grad_scale=scale)
@@ -87,13 +91,20 @@ if world > 1:
 ms = float(ms)
 n_train = sum(p.numel() for p in all_params)
 if rank == 0:
-    print(json.dumps({"metric": "pdae_training_images_per_sec", "value": round(world * B / ms * 1e3, 2), "unit": "images/s",
-                      "n_gpus": world, "batch_per_gpu": B, "ms_per_step": round(ms, 2), "steps": args.steps, "warmup": 3,
-                      "scaling": "weak", "grad_allreduce": ("overlapped with the encoder backward" if red is not None else
-                                                            ("after backward" if world > 1 else "none (1 GPU)")),
-                      "trainable_params": n_train, "allreduce_bytes_per_step": 4 * n_train if world > 1 else 0,
-                      "config": "celeba64-proxy encoder + ShiftUNet (shift half trainable), dropout 0.1, fused Adam+EMA; decoder "
-                                "forward, data and weight gradients on the tensor cores (split-operand, fp32-grade); encoder "
-                                "and stride-2 / 3-channel convs on CUDA cores (fp32)", "loss": float(loss.detach())}))
+    res = {"metric": "pdae_training_images_per_sec", "value": round(world * B / ms * 1e3, 2), "unit": "images/s",
+           "n_gpus": world, "batch_per_gpu": B, "ms_per_step": round(ms, 2), "steps": args.steps, "warmup": 3,
+           "scaling": "weak", "grad_allreduce": ("overlapped with the encoder backward" if red is not None else
+                                                 ("after backward" if world > 1 else "none (1 GPU)")),
+           "trainable_params": n_train, "allreduce_bytes_per_step": 4 * n_train if world > 1 else 0,
+           "config": "celeba64-proxy encoder + ShiftUNet (shift half trainable), dropout 0.1, fused Adam+EMA; decoder "
+                     "forward, data and weight gradients on the tensor cores (split-operand, fp32-grade); encoder "
+                     "and stride-2 / 3-channel convs on CUDA cores (fp32)", "loss": float(loss.detach())}
+    if args.amp != "off":
+        res["amp"] = args.amp
+        res["config"] = ("celeba64-proxy encoder + ShiftUNet (shift half trainable), dropout 0.1, fused Adam+EMA, bf16 autocast; "
+                         "frozen decoder half in bf16, trainable decoder forward, data and weight gradients as single-pass "
+                         "bf16 MMAs on the tensor cores; fp32 activations, GroupNorm and attention backward; encoder and "
+                         "stride-2 / 3-channel convs on CUDA cores (fp32)")
+    print(json.dumps(res))
 if world > 1:
     dist.destroy_process_group()

@@ -1,5 +1,5 @@
-"""Micro-benchmark of wgrad_tc vs conv2d_wgrad_simt on the celeba64-proxy training shapes (B=32).
-usage: python scripts/wgrad_bench.py"""
+"""Micro-benchmark of wgrad_tc (split-operand and single-pass bf16) vs conv2d_wgrad_simt on the celeba64-proxy training shapes
+(B=32).  usage: python scripts/wgrad_bench.py"""
 import ctypes
 import os
 import sys
@@ -40,16 +40,23 @@ for (B, H, W, Cin, Cout, k) in [(32, 32, 32, 128, 128, 3), (32, 32, 32, 256, 128
     dw = torch.zeros(k * k, Cin, Cout, device=DEV)
     dw2 = torch.zeros_like(dw)
     a3, d3 = split3(act), split3(dy)
+    ab, db = act.to(torch.bfloat16), dy.to(torch.bfloat16)
+    dwb = torch.zeros_like(dw)
     st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-    h = ctypes.c_void_p()
+    h, hb = ctypes.c_void_p(), ctypes.c_void_p()
     _native.check(L.pdae_wgrad_tc_create(ctypes.byref(h), p(a3), p(d3), p(dw), B, H, W, Cin, Cout, k), "create")
+    _native.check(L.pdae_wgrad_tc_create_bf16(ctypes.byref(hb), p(ab), p(db), p(dwb), B, H, W, Cin, Cout, k), "create_bf16")
     t_tc = timeit(lambda: _native.check(L.pdae_wgrad_tc_run(h, st), "run"))
+    t_bf = timeit(lambda: _native.check(L.pdae_wgrad_tc_run(hb, st), "run bf16"))
     t_simt = timeit(lambda: _native.check(L.pdae_conv2d_wgrad_simt(p(act), 0, 0, p(dy), p(dw2), B, H, W, Cin, Cout, k, 1, k // 2, st), "simt"), 3)
-    dw.zero_(); dw2.zero_()
-    L.pdae_wgrad_tc_run(h, st); L.pdae_conv2d_wgrad_simt(p(act), 0, 0, p(dy), p(dw2), B, H, W, Cin, Cout, k, 1, k // 2, st)
+    dw.zero_(); dw2.zero_(); dwb.zero_()
+    L.pdae_wgrad_tc_run(h, st); L.pdae_wgrad_tc_run(hb, st)
+    L.pdae_conv2d_wgrad_simt(p(act), 0, 0, p(dy), p(dw2), B, H, W, Cin, Cout, k, 1, k // 2, st)
     torch.cuda.synchronize()
     rel = ((dw - dw2).abs().max() / dw2.abs().max()).item()
+    rel_b = ((dwb - dw2).abs().max() / dw2.abs().max()).item()
     fl = 2.0 * B * H * W * Cin * Cout * k * k
     print(f"B{B} {H}x{W} {Cin}->{Cout} k{k}: wgrad_tc {t_tc:8.1f} us ({fl / t_tc / 1e6:7.1f} TF alg, {3 * fl / t_tc / 1e6:7.1f} exec)   "
-          f"simt {t_simt:8.1f} us   rel diff {rel:.2e}", flush=True)
+          f"bf16 {t_bf:8.1f} us ({fl / t_bf / 1e6:7.1f} TF)   simt {t_simt:8.1f} us   rel diff {rel:.2e} (bf16 {rel_b:.2e})", flush=True)
     L.pdae_wgrad_tc_destroy(h)
+    L.pdae_wgrad_tc_destroy(hb)
