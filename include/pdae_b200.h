@@ -211,6 +211,11 @@ int pdae_wgrad_tc_create(pdae_wgrad_tc_plan** plan, const void* act3_bf16, const
  * is one bf16 MMA with fp32 accumulation.  Same shapes, zeroing contract and run / destroy functions as above. */
 int pdae_wgrad_tc_create_bf16(pdae_wgrad_tc_plan** plan, const void* act_bf16, const void* dy_bf16, float* dw, int B, int H, int W,
                               int Cin, int Cout, int ksize);
+/* Weight gradient of a 3x3, stride-2, pad-1 conv on plain bf16 operands (the semantic encoder under autocast):
+ * dw[3 ky + kx][cin][cout] += sum_{b,oy,ox} act[b, 2 oy + ky - 1, 2 ox + kx - 1, cin] * dy[b, oy, ox, cout].  act: [B][H][W][Cin],
+ * dy: [B][H/2][W/2][Cout], H and W even, channels as pdae_conv_s2_tc_supported.  Same zeroing contract and run / destroy. */
+int pdae_wgrad_tc_create_bf16_s2(pdae_wgrad_tc_plan** plan, const void* act_bf16, const void* dy_bf16, float* dw, int B, int H,
+                                 int W, int Cin, int Cout);
 int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* plan, pdae_stream_t stream);
 void pdae_wgrad_tc_destroy(pdae_wgrad_tc_plan* plan);
 
@@ -248,6 +253,16 @@ int pdae_gemm_tc2_create(pdae_conv_tc2_plan** plan, const void* a_bf16, long lon
 int pdae_gemm_tc2_softmax_create(pdae_conv_tc2_plan** plan, const void* a_bf16, long long a_ld, long long a_bs,
                                  const void* b_bf16, long long b_ld, long long b_bs, void* out_bf16, long long out_ld,
                                  long long out_bs, int batch, int M, int N, int K, float alpha);
+/* 3x3, stride-2, pad-1 convs on plain bf16 operands with fp32 accumulation (the semantic encoder's training step under
+ * autocast, model/representation_learning/encoder).  H, W: the conv's input size, both even; Cin % 64 == 0, Cout % 64 == 0
+ * (pdae_conv_s2_tc_supported).  Forward: out[B][H/2][W/2][Cout] fp32 = conv(in[B][H][W][Cin] bf16, w[9][Cout][Cin] bf16)
+ * + bias (optional).  Data gradient: dx[B][H][W][Cin] fp32 (every element written) from dy[B][H/2][W/2][Cout] bf16 and
+ * wt[9][Cin][Cout] bf16, wt[3 ky + kx][ci][co] = w[co][ci][ky][kx] (transposed, not flipped).  Run / destroy as above.  */
+int pdae_conv_s2_tc_supported(int H, int W, int Cin, int Cout);
+int pdae_conv_tc2_create_s2(pdae_conv_tc2_plan** plan, const void* in_bf16, const void* w_bf16, const float* bias, float* out,
+                            int B, int H, int W, int Cin, int Cout);
+int pdae_conv_tc2_create_s2_dgrad(pdae_conv_tc2_plan** plan, const void* dy_bf16, const void* wt_bf16, float* dx, int B, int H,
+                                  int W, int Cin, int Cout);
 int pdae_conv_tc2_run(const pdae_conv_tc2_plan* plan, pdae_stream_t stream);
 /* Image-head plans (cout_valid > 0): fuse the per-step DDIM update (diffusion/ddim.py:43-55,66-79,91-107,123-138) into the head's
  * epilogue.  fuse_desc_device: 8 x int64 in DEVICE memory, read at run time = { flags, eps*, x_t*, t*, tab_A*, tab_Bm*, tab_s1m*,

@@ -98,6 +98,9 @@ _SIGS = {
                                      c_int, c_int, c_int, c_int]),
     "pdae_gemm_tc2_softmax_create": (c_int, [POINTER(c_void_p), _P, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int64, c_int64,
                                              c_int, c_int, c_int, c_int, c_float]),
+    "pdae_conv_s2_tc_supported": (c_int, [c_int, c_int, c_int, c_int]),
+    "pdae_conv_tc2_create_s2": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_conv_tc2_create_s2_dgrad": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_run": (c_int, [_P, _P]),
     "pdae_conv_tc2_set_head_fuse": (c_int, [_P, _P]),
     "pdae_conv_tc3_supported": (c_int, [c_int, c_int, c_int, c_int]),
@@ -108,6 +111,7 @@ _SIGS = {
     "pdae_wgrad_tc_supported": (c_int, [c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_create": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_create_bf16": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_wgrad_tc_create_bf16_s2": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_run": (c_int, [_P, _P]),
     "pdae_wgrad_tc_destroy": (None, [_P]),
     "pdae_softmax_bf16": (c_int, [_P, _P, c_int64, c_int, c_float, _P]),

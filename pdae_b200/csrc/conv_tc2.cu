@@ -10,6 +10,17 @@
 //
 // The BN=16 instantiation is the UNet image head (Cout=3 zero-padded to 16): it skips the TMA store and writes the
 // first `cout_valid` columns as NCHW fp32 planes.
+//
+// S2 != 0: the three-by-three, stride-2, pad-1 convs of the semantic encoder (bf16 autocast training).  An NHWC tensor
+// [B][H][W][C] is addressed through its PARITY VIEW, the same memory as [B][H/2][2][W/2][2C]: pixel (2 a + py, 2 b + px),
+// channel c sits at the 5-D TMA coordinate (px C + c, b, py, a, image).  Each parity class is a dense stride-1 grid.
+//   S2 = 1, forward: output row o reads input row 2 o + ky - 1 = parity (ky != 1) at row o - (ky == 0), so each tap is a box
+//           of one parity class at the output tile shifted by -1 or 0; the only out-of-range coordinate is -1, whose TMA zero
+//           fill is the padding.  The tiles cover the output grid, the epilogue is the ordinary one (bias, fp32 store).
+//   S2 = 2, data gradient as four sub-pixel phases: dX at parity (py, px) is a stride-1 correlation of dY with the taps
+//           ky = 1 (py = 0) or ky = 0 at dY row + 1 and ky = 2 at dY row + 0 (py = 1), likewise kx: 1, 2, 2 or 4 taps, 9 over
+//           the four phases (the forward's MMA count).  The phase is the fastest tile index, so every CTA's contiguous tile
+//           range mixes the cheap and the expensive phases; each tile is stored through the parity view of dX.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -106,6 +117,19 @@ __device__ __forceinline__ void tma_st4(const CUtensorMap* m, uint32_t src, int 
                "r"(c0), "r"(c1), "r"(c2), "r"(c3)
                : "memory");
 }
+__device__ __forceinline__ void tma_ld5(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+      ::"r"(dst), "l"(m), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
+__device__ __forceinline__ void tma_st5(const CUtensorMap* m, uint32_t src, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile("cp.async.bulk.tensor.5d.global.shared::cta.bulk_group [%0, {%2, %3, %4, %5, %6}], [%1];" ::"l"(m), "r"(src),
+               "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+               : "memory");
+}
+// stride-2 data gradient: number of taps of sub-pixel phase (py, px) = ph (py = ph >> 1, px = ph & 1)
+__device__ __forceinline__ int s2_phase_taps(int ph) { return (1 + (ph >> 1)) * (1 + (ph & 1)); }
 // One elected lane of a fully converged warp: the producer / issuer loops run on all 32 lanes (warp-uniform operands stay in
 // uniform registers); only the TMA instruction is predicated.  Under `if (lane == 0)` every descriptor was a
 // per-lane value and each MMA paid an ELECT + 5 x R2UR.BROADCAST + branch waterfall.
@@ -120,7 +144,7 @@ __device__ __forceinline__ void cons_bar() { asm volatile("bar.sync 1, 256;" :::
 // byte offset of (row, 16-byte chunk) inside a 128-row x 128-byte SWIZZLE_128B staging tile
 __device__ __forceinline__ uint32_t swz(int row, int chunk16) { return (uint32_t)(row * 128 + ((chunk16 ^ (row & 7)) << 4)); }
 
-template <int BN, bool OB>
+template <int BN, bool OB, int S2 = 0>
 __global__ void __launch_bounds__(T2_THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
@@ -188,13 +212,44 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       __syncwarp();
     }
     for (int tile = tile_begin; tile < tile_end; ++tile) {
-      const int nt = tile / p.tiles_m;
-      int mt = tile - nt * p.tiles_m;
+      const int ph2 = S2 == 2 ? (tile & 3) : 0;      // stride-2 dgrad: sub-pixel phase of this tile
+      const int tl = S2 == 2 ? (tile >> 2) : tile;
+      const int nt = tl / p.tiles_m;
+      int mt = tl - nt * p.tiles_m;
       const int tx = mt % p.tiles_x;
       mt /= p.tiles_x;
       const int ty = mt % p.tiles_y;
       const int bt = mt / p.tiles_y;
       const int x0 = tx * p.tw, y0 = ty * p.th, b0 = bt * p.tn, n0 = nt * BN;
+      if constexpr (S2 != 0) {
+        const int cin = p.kblocks * T2_BK;
+        const int nx = 1 + (ph2 & 1);
+        const int n_it = (S2 == 1 ? 9 : s2_phase_taps(ph2)) * p.kblocks;
+        for (int it = 0; it < n_it; ++it) {
+          const int j = it / p.kblocks, kb = it - j * p.kblocks;
+          mb_wait(s_u32(&bar_empty[s]), ph ^ 1u);
+          const uint32_t full = s_u32(&bar_full[s]);
+          const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
+          if (elect_one()) {
+            mb_expect_tx(full, stage_tx);
+            int wtap;
+            if (S2 == 1) {           // forward tap j = (ky, kx): parity (ky != 1, kx != 1) at the output tile - (k == 0)
+              const int ky = j / 3, kx = j - 3 * ky;
+              wtap = j;
+              tma_ld5(sa, &tmA, full, (kx != 1) * cin + kb * T2_BK, x0 - (kx == 0), ky != 1, y0 - (ky == 0), b0);
+            } else {                 // dgrad phase (py, px), tap j: ky = 1 (py = 0) or 0 / 2 at dY row + 1 / + 0 (py = 1)
+              const int jy = j / nx, jx = j - jy * nx;
+              const int ky = (ph2 >> 1) ? 2 * jy : 1, kx = (ph2 & 1) ? 2 * jx : 1;
+              wtap = 3 * ky + kx;
+              tma_ld4(sa, &tmA, full, kb * T2_BK, x0 + (kx == 0), y0 + (ky == 0), b0);
+            }
+            if (!ws) tma_ld3(sa + T2_A_BYTES, &tmB, full, kb * T2_BK, n0, wtap);
+          }
+          __syncwarp();
+          if (++s == S) { s = 0; ph ^= 1u; }
+        }
+        continue;
+      }
       int tap = 0, kb = 0, dy = p.ksize == 3 ? -1 : 0, dx = dy;
       for (int it = 0; it < total_k; ++it) {
         mb_wait(s_u32(&bar_empty[s]), ph ^ 1u);
@@ -244,13 +299,16 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     for (int i = 0; i < BN / 2; ++i) acc[i] = 0.f;
     if (p.w_stat && tile_begin < tile_end) mb_wait(s_u32(&bar_w), 0u);   // stationary weights have landed
     for (int tile = tile_begin; tile < tile_end; ++tile) {
-      const int nt = tile / p.tiles_m;
-      int mt = tile - nt * p.tiles_m;
+      const int ph2 = S2 == 2 ? (tile & 3) : 0;
+      const int tl = S2 == 2 ? (tile >> 2) : tile;
+      const int nt = tl / p.tiles_m;
+      int mt = tl - nt * p.tiles_m;
       const int tx = mt % p.tiles_x;
       mt /= p.tiles_x;
       const int ty = mt % p.tiles_y;
       const int bt = mt / p.tiles_y;
       const int x0 = tx * p.tw, y0 = ty * p.th, b0 = bt * p.tn, n0 = nt * BN;
+      const int n_it = S2 == 2 ? s2_phase_taps(ph2) * p.kblocks : total_all;
       if constexpr (BN != 16) {
         if (p.has_res && elected) {            // residual chunk 0 of this tile (lands while the main loop runs)
           mb_expect_tx(rbar, T2_STG_BYTES);
@@ -259,7 +317,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       }
       // ---- main loop: wgmma over the stage ring; a stage is released once the MMAs reading it have retired ----
       int prev = -1;
-      for (int it = 0; it < total_all; ++it) {
+      for (int it = 0; it < n_it; ++it) {
         mb_wait(s_u32(&bar_full[s]), ph);
         const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
         const uint64_t ad = wgmma::desc_sw128(sa + (uint32_t)wg * (64u * 128u), 16u, 1024u);
@@ -395,7 +453,8 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           asm volatile("fence.proxy.async.shared::cta;" ::: "memory");
           cons_bar();
           if (elected) {
-            tma_st4(&tmO, obuf, n0 + c * CW, x0, y0, b0);
+            if constexpr (S2 == 2) tma_st5(&tmO, obuf, (ph2 & 1) * p.Cout + n0 + c * CW, x0, ph2 >> 1, y0, b0);   // dX parity view
+            else tma_st4(&tmO, obuf, n0 + c * CW, x0, y0, b0);
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
           }
           if (p.ch_stats) {
@@ -532,17 +591,17 @@ static int pow2_tile(int W, int cap) {
   return t;
 }
 
-template <int BN, bool OB>
+template <int BN, bool OB, int S2 = 0>
 static cudaError_t launch_tc2(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r,
                               const CUtensorMap& a2, const CUtensorMap& b2, const CUtensorMap& a3, const ConvTc2Args& args,
                               int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, OB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, stats <= 2 KB) <= 227 KB
+    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, OB, S2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, stats <= 2 KB) <= 227 KB
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  conv_tc2_kernel<BN, OB><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args);
+  conv_tc2_kernel<BN, OB, S2><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args);
   return cudaPeekAtLastError();
 }
 
@@ -554,6 +613,7 @@ struct pdae_conv_tc2_plan {
   CUtensorMap tmA, tmB, tmO, tmR, tmA2, tmB2, tmA3;
   ConvTc2Args args;
   int BN, grid;
+  int s2;           // 0: stride-1 conv / GEMM; 1: stride-2 forward; 2: stride-2 data gradient (conv_tc2_kernel's S2)
   size_t smem;
 };
 
@@ -571,6 +631,8 @@ struct Tc2Desc {
   const void* in2 = nullptr; const void* w2 = nullptr; int Cin2 = 0;   // fused 1x1 skip conv (bf16 NHWC input, [Cout][Cin2] weights)
   float softmax_alpha = 0.f;  // batched GEMM only: store softmax_row(alpha * out) as bf16 (needs N == BN)
   const void* in3 = nullptr; int Cin2a = 0;   // skip input = channel concat of in2 [..,Cin2a] and in3 [..,Cin2-Cin2a] (in3 == nullptr: in2 alone)
+  int s2 = 0;   // stride-2 3x3 conv (kernel header): H, W are the OUTPUT / dY grid; 1: `in` is read through its parity view;
+                // 2: data gradient, `out` (fp32 dX) is written through its parity view
 };
 
 static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
@@ -631,7 +693,8 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
     PDAE_REQUIRE(false, "conv_tc2_create: Cout=%d not a multiple of BN=%d", Cout, BN);
   }
   pl->BN = BN;
-  a.tiles_total = a.tiles_m * (head ? 1 : Cout / BN);
+  pl->s2 = d.s2;
+  a.tiles_total = a.tiles_m * (head ? 1 : Cout / BN) * (d.s2 == 2 ? 4 : 1);   // stride-2 dgrad: x 4 sub-pixel phases
   const int b_bytes = ((BN * T2_BK * 2 + 1023) / 1024) * 1024;
   int stage_bytes = T2_A_BYTES + b_bytes;
   const int staging = head ? 0 : (a.has_res ? 2 : 1) * T2_STG_BYTES;
@@ -642,7 +705,8 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
   // 64-channel layers are L2->SM bandwidth-bound: this removes a third of their bytes).
   int wbytes = 0;
   a.w_stat = 0;
-  if (!head && !d.w_batched && Cout == BN && b_bytes == BN * T2_BK * 2 && a.tiles_total >= 2 * pl->grid) {
+  // (not for the stride-2 dgrad: its phases read different subsets of the taps)
+  if (!head && !d.w_batched && d.s2 != 2 && Cout == BN && b_bytes == BN * T2_BK * 2 && a.tiles_total >= 2 * pl->grid) {
     const int wb = total_all * b_bytes;
     if ((220 * 1024 - 1024 - staging - wb) / T2_A_BYTES >= 4) {
       a.w_stat = 1;
@@ -663,7 +727,18 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
     return PDAE_EINVAL;
   };
   cuuint32_t estr4[4] = {1, 1, 1, 1};
-  {
+  cuuint32_t estr5[5] = {1, 1, 1, 1, 1};
+  if (d.s2 == 1) {
+    // parity view of the [B][2H][2W][Cin] input: [B][H][2][W][2 Cin] (kernel header); box = one parity class of the tile
+    const cuuint64_t c2 = 2ull * Cin;
+    cuuint64_t dims[5] = {c2, (cuuint64_t)W, 2, (cuuint64_t)H, (cuuint64_t)B};
+    cuuint64_t strides[4] = {c2 * 2, 2 * W * c2, 2 * W * c2 * 2, (cuuint64_t)H * 2 * W * c2 * 2};
+    cuuint32_t box[5] = {(cuuint32_t)T2_BK, (cuuint32_t)a.tw, 1, (cuuint32_t)a.th, (cuuint32_t)a.tn};
+    CUresult r = enc(&pl->tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(d.in), dims, strides, box, estr5,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail("A (parity view)", (int)r);
+  } else {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)d.in_ld * 2, (cuuint64_t)W * d.in_ld * 2, (cuuint64_t)d.in_bs * 2};
     cuuint32_t box[4] = {(cuuint32_t)T2_BK, (cuuint32_t)a.tw, (cuuint32_t)a.th, (cuuint32_t)a.tn};
@@ -714,7 +789,16 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
             CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail("W2", (int)r);
   }
-  if (!head) {
+  if (d.s2 == 2) {
+    // parity view of the fp32 [B][2H][2W][Cout] data gradient: [B][H][2][W][2 Cout]; one phase per store box
+    const cuuint64_t c2 = 2ull * Cout;
+    cuuint64_t dims[5] = {c2, (cuuint64_t)W, 2, (cuuint64_t)H, (cuuint64_t)B};
+    cuuint64_t strides[4] = {c2 * 4, 2 * W * c2 * 2, 2 * W * c2 * 4, (cuuint64_t)H * 2 * W * c2 * 4};
+    cuuint32_t box[5] = {32, (cuuint32_t)a.tw, 1, (cuuint32_t)a.th, (cuuint32_t)a.tn};
+    CUresult r = enc(&pl->tmO, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 5, d.out, dims, strides, box, estr5, CU_TENSOR_MAP_INTERLEAVE_NONE,
+                     CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_NONE, CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail("O (parity view)", (int)r);
+  } else if (!head) {
     const int esz = a.out_bf16 ? 2 : 4;
     cuuint64_t dims[4] = {(cuuint64_t)Cout, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)d.out_ld * esz, (cuuint64_t)W * d.out_ld * esz, (cuuint64_t)d.out_bs * esz};
@@ -814,19 +898,77 @@ extern "C" int pdae_gemm_tc2_softmax_create(pdae_conv_tc2_plan** plan_out, const
   return tc2_create(plan_out, d);
 }
 
+// ---- 3x3, stride-2, pad-1 convs on plain bf16 operands (the semantic encoder's bf16 autocast training step) ----------------
+// H, W: the conv's INPUT size (even); the output / dY grid is H/2 x W/2.  Every tile shape the 128- and 64-pixel boxes of
+// conv_tc2 / wgrad_tc need exists for such a grid (power-of-two tiles, several images per box when the grid is small).
+extern "C" int pdae_conv_s2_tc_supported(int H, int W, int Cin, int Cout) {
+  return H >= 2 && W >= 2 && H % 2 == 0 && W % 2 == 0 && Cin >= 64 && Cout >= 64 && Cin % 64 == 0 && Cout % 64 == 0;
+}
+
+static int s2_validate(const char* fn, const void* a, const void* b, const void* out, const float* bias, int B, int H, int W,
+                       int Cin, int Cout) {
+  PDAE_REQUIRE(a && b && out, "%s: null pointer", fn);
+  PDAE_REQUIRE(!(((uintptr_t)a | (uintptr_t)b | (uintptr_t)out | (uintptr_t)bias) & 15), "%s: pointers must be 16-byte aligned", fn);
+  PDAE_REQUIRE(B > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0, "%s: B=%d H=%d W=%d: H and W must be even and positive", fn, B,
+               H, W);
+  PDAE_REQUIRE(pdae_conv_s2_tc_supported(H, W, Cin, Cout), "%s: unsupported channels Cin=%d Cout=%d (multiples of 64)", fn, Cin,
+               Cout);
+  return PDAE_OK;
+}
+
+// out[B][H/2][W/2][Cout] (fp32) = conv3x3_stride2_pad1(in[B][H][W][Cin] (bf16), w[9][Cout][Cin] (bf16)) + bias
+extern "C" int pdae_conv_tc2_create_s2(pdae_conv_tc2_plan** plan_out, const void* in_bf16, const void* w_bf16, const float* bias,
+                                       float* out, int B, int H, int W, int Cin, int Cout) {
+  PDAE_REQUIRE(plan_out, "conv_tc2_create_s2: null pointer");
+  const int rc = s2_validate("conv_tc2_create_s2", in_bf16, w_bf16, out, bias, B, H, W, Cin, Cout);
+  if (rc != PDAE_OK) return rc;
+  const int Ho = H / 2, Wo = W / 2;
+  Tc2Desc d;
+  d.in = in_bf16; d.w = w_bf16; d.bias = bias; d.residual = nullptr; d.out = out; d.out_dtype = PDAE_F32;
+  d.ch_stats = nullptr; d.B = B; d.H = Ho; d.W = Wo; d.Cin = Cin; d.Cout = Cout; d.ksize = 3; d.cout_valid = 0; d.bn_override = 0;
+  d.in_ld = Cin; d.in_bs = (long long)H * W * Cin;
+  d.w_batched = 0; d.w_ld = Cin; d.w_bs = (long long)Cout * Cin;
+  d.out_ld = Cout; d.out_bs = (long long)Ho * Wo * Cout;
+  d.s2 = 1;
+  return tc2_create(plan_out, d);
+}
+
+// Data gradient of the same conv: dx[B][H][W][Cin] (fp32, every element written) from dy[B][H/2][W/2][Cout] (bf16) and the
+// transposed weights wt[9][Cin][Cout] (bf16, wt[3 ky + kx][ci][co] = w[co][ci][ky][kx], NOT flipped: the phases pick the taps)
+extern "C" int pdae_conv_tc2_create_s2_dgrad(pdae_conv_tc2_plan** plan_out, const void* dy_bf16, const void* wt_bf16, float* dx,
+                                             int B, int H, int W, int Cin, int Cout) {
+  PDAE_REQUIRE(plan_out, "conv_tc2_create_s2_dgrad: null pointer");
+  const int rc = s2_validate("conv_tc2_create_s2_dgrad", dy_bf16, wt_bf16, dx, nullptr, B, H, W, Cin, Cout);
+  if (rc != PDAE_OK) return rc;
+  const int Ho = H / 2, Wo = W / 2;
+  Tc2Desc d;   // a GEMM over the dY grid with K = Cout, N = Cin
+  d.in = dy_bf16; d.w = wt_bf16; d.bias = nullptr; d.residual = nullptr; d.out = dx; d.out_dtype = PDAE_F32;
+  d.ch_stats = nullptr; d.B = B; d.H = Ho; d.W = Wo; d.Cin = Cout; d.Cout = Cin; d.ksize = 3; d.cout_valid = 0; d.bn_override = 0;
+  d.in_ld = Cout; d.in_bs = (long long)Ho * Wo * Cout;
+  d.w_batched = 0; d.w_ld = Cout; d.w_bs = (long long)Cin * Cout;
+  d.out_ld = Cin; d.out_bs = (long long)H * W * Cin;
+  d.s2 = 2;
+  return tc2_create(plan_out, d);
+}
+
 extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t stream) {
   PDAE_REQUIRE(pl, "conv_tc2_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
 #define T2_GO(BN, OB) launch_tc2<BN, OB>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s)
+#define T2_GO_S2(BN, S2) \
+  launch_tc2<BN, false, S2>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s)
   const bool ob = pl->args.out_bf16 != 0;
-  switch (pl->BN) {
+  if (pl->s2 == 1) e = pl->BN == 128 ? T2_GO_S2(128, 1) : T2_GO_S2(64, 1);
+  else if (pl->s2 == 2) e = pl->BN == 128 ? T2_GO_S2(128, 2) : T2_GO_S2(64, 2);
+  else switch (pl->BN) {
     case 16: e = T2_GO(16, false); break;
     case 64: e = ob ? T2_GO(64, true) : T2_GO(64, false); break;
     case 128: e = ob ? T2_GO(128, true) : T2_GO(128, false); break;
     default: e = ob ? T2_GO(256, true) : T2_GO(256, false); break;
   }
 #undef T2_GO
+#undef T2_GO_S2
   if (e != cudaSuccess) {
     (void)cudaGetLastError();
     set_error("launch of conv_tc2_kernel<%d> failed: %s", pl->BN, cudaGetErrorString(e));

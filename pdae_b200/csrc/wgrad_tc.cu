@@ -25,6 +25,11 @@
 // Cout % 128 == 0.  When neither channel count is a
 // multiple of 128 (64 -> 64, 192 -> 64) the M side is the activation in 64-channel chunks and the two 64-row halves of the
 // accumulator hold two different TAPS of it ("pair" mode; the odd ninth tap is paired with a discarded duplicate).
+//
+// S2 = true: a 3x3, stride-2, pad-1 conv on plain bf16 operands (the semantic encoder under autocast).  The pixel tiles cover
+// the OUTPUT grid (dY is read there, unshifted); the activation is read through its parity view [B][H/2][2][W/2][2C]
+// (conv_tc2.cu): tap (ky, kx) is the parity class (ky != 1, kx != 1) at the output tile shifted by -1 where the tap index is
+// 0, the -1 coordinate being zero-filled by TMA (the padding).
 #include <cuda.h>
 
 #include "common.cuh"
@@ -85,6 +90,18 @@ __device__ __forceinline__ void tma_ld4(uint32_t dst, const CUtensorMap* m, uint
       ::"r"(dst), "l"(m), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3)
       : "memory");
 }
+__device__ __forceinline__ void tma_ld5(uint32_t dst, const CUtensorMap* m, uint32_t bar, int c0, int c1, int c2, int c3, int c4) {
+  asm volatile(
+      "cp.async.bulk.tensor.5d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%3, %4, %5, %6, %7}], [%2];"
+      ::"r"(dst), "l"(m), "r"(bar), "r"(c0), "r"(c1), "r"(c2), "r"(c3), "r"(c4)
+      : "memory");
+}
+// stride-2 activation box of tap `tap` (ky = tap / 3, kx = tap % 3) at channel c of a C-channel tensor, output tile (x0, y0, b0)
+__device__ __forceinline__ void tma_ld_s2(uint32_t dst, const CUtensorMap* m, uint32_t bar, int C, int c, int tap, int x0, int y0,
+                                          int b0) {
+  const int ky = tap / 3, kx = tap - 3 * ky;
+  tma_ld5(dst, m, bar, (kx != 1) * C + c, x0 - (kx == 0), ky != 1, y0 - (ky == 0), b0);
+}
 __device__ __forceinline__ bool elect_one() {
   uint32_t pred;
   asm volatile("{\n\t.reg .pred p;\n\telect.sync _|p, 0xffffffff;\n\tselp.b32 %0, 1, 0, p;\n\t}" : "=r"(pred));
@@ -92,10 +109,11 @@ __device__ __forceinline__ bool elect_one() {
 }
 }  // namespace wg
 
-template <int BN, bool SPLIT>
+template <int BN, bool SPLIT, bool S2 = false>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, WgradArgs p) {
   using namespace wg;
+  static_assert(!(SPLIT && S2), "stride-2 weight gradients take plain bf16 operands");
   extern __shared__ uint8_t smem_raw[];
   constexpr int MAX_ST = SPLIT ? WG_MAX_ST : WG_MAX_ST_BF16;
   __shared__ __align__(8) uint64_t bar_full[MAX_ST], bar_empty[MAX_ST];
@@ -154,7 +172,23 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       mb_wait(s_u32(&bar_empty[s]), ph ^ 1u);
       const uint32_t full = s_u32(&bar_full[s]);
       const uint32_t base = smem0 + (uint32_t)(s * STAGE);
-      if (elect_one()) {
+      if constexpr (S2) {
+        if (elect_one()) {
+          mb_expect_tx(full, (uint32_t)STAGE);
+#pragma unroll
+          for (int j = 0; j < 2; ++j) {
+            const uint32_t dst = base + (uint32_t)(j * WG_BOX);
+            if (p.a_is_act) tma_ld_s2(dst, &tmA, full, p.Ma, am[j], tj[j], x0, y0, b0);
+            else tma_ld4(dst, &tmA, full, am[j], x0, y0, b0);
+          }
+#pragma unroll
+          for (int j = 0; j < NBOX_B; ++j) {
+            const uint32_t dst = base + (uint32_t)(A_BYTES + j * WG_BOX);
+            if (p.a_is_act) tma_ld4(dst, &tmB, full, n0 + j * 64, x0, y0, b0);
+            else tma_ld_s2(dst, &tmB, full, p.Nb, n0 + j * 64, tap, x0, y0, b0);
+          }
+        }
+      } else if (elect_one()) {
         mb_expect_tx(full, (uint32_t)STAGE);
 #pragma unroll
         for (int h = 0; h < NBLK; ++h) {       // hi block (channel offset 0), lo block (channel offset Ma / Nb)
@@ -257,15 +291,15 @@ static int pow2_tile_w(int W, int cap) {
   return t;
 }
 
-template <int BN, bool SPLIT>
+template <int BN, bool SPLIT, bool S2 = false>
 static cudaError_t launch_wg(const CUtensorMap& a, const CUtensorMap& b, const WgradArgs& args, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<BN, SPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<BN, SPLIT, S2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  wgrad_tc_kernel<BN, SPLIT><<<grid, WG_THREADS, smem, s>>>(a, b, args);
+  wgrad_tc_kernel<BN, SPLIT, S2><<<grid, WG_THREADS, smem, s>>>(a, b, args);
   return cudaPeekAtLastError();
 }
 
@@ -277,6 +311,7 @@ struct pdae_wgrad_tc_plan {
   CUtensorMap tmA, tmB;
   WgradArgs args;
   int BN, split, grid;
+  int s2;           // stride-2 3x3 conv (wgrad_tc_kernel's S2)
   size_t smem;
 };
 
@@ -290,14 +325,24 @@ extern "C" int pdae_wgrad_tc_supported(int H, int W, int Cin, int Cout, int ksiz
   return (W % tw == 0 && H % th == 0 && tw * th * tn == WG_KT && tn <= 64) ? 1 : 0;
 }
 
-// split: act / dy hold [hi | lo | hi] blocks of 3*C channels; otherwise plain bf16 with C channels
+// split: act / dy hold [hi | lo | hi] blocks of 3*C channels; otherwise plain bf16 with C channels.
+// s2: 3x3 stride-2 pad-1 conv, H x W = the activation's size, dy on the H/2 x W/2 grid (plain bf16 only)
 static int wgrad_create(pdae_wgrad_tc_plan** plan_out, const void* act, const void* dy, float* dw, int B, int H, int W, int Cin,
-                        int Cout, int ksize, bool split) {
+                        int Cout, int ksize, bool split, bool s2 = false) {
   PDAE_REQUIRE(plan_out && act && dy && dw, "wgrad_tc_create: null pointer");
-  PDAE_REQUIRE(pdae_wgrad_tc_supported(H, W, Cin, Cout, ksize), "wgrad_tc_create: unsupported shape H=%d W=%d Cin=%d Cout=%d k=%d", H, W,
-               Cin, Cout, ksize);
+  if (s2) {
+    PDAE_REQUIRE(B > 0 && H > 0 && W > 0 && H % 2 == 0 && W % 2 == 0,
+                 "wgrad_tc_create_bf16_s2: B=%d H=%d W=%d: H and W must be even and positive", B, H, W);
+    PDAE_REQUIRE(ksize == 3 && !split && pdae_conv_s2_tc_supported(H, W, Cin, Cout),
+                 "wgrad_tc_create_bf16_s2: unsupported channels Cin=%d Cout=%d (multiples of 64)", Cin, Cout);
+  } else {
+    PDAE_REQUIRE(pdae_wgrad_tc_supported(H, W, Cin, Cout, ksize), "wgrad_tc_create: unsupported shape H=%d W=%d Cin=%d Cout=%d k=%d", H, W,
+                 Cin, Cout, ksize);
+  }
   PDAE_REQUIRE(!(((uintptr_t)act | (uintptr_t)dy) & 15) && !((uintptr_t)dw & 3),
                "wgrad_tc_create: act / dy must be 16-byte aligned (TMA), dw 4-byte aligned");
+  const int Ha = H, Wa = W;          // activation size
+  if (s2) { H /= 2; W /= 2; }        // from here on: the pixel grid the tiles cover (dY's)
   EncodeTiledFnW enc = encode_fnw();
   PDAE_REQUIRE(enc != nullptr, "wgrad_tc_create: cuTensorMapEncodeTiled unavailable (no driver)");
   if (g_num_sms_w == 0) {
@@ -318,6 +363,7 @@ static int wgrad_create(pdae_wgrad_tc_plan** plan_out, const void* act, const vo
   const int BN = (a.Nb % 128 == 0) ? 128 : 64;
   pl->BN = BN;
   pl->split = split ? 1 : 0;
+  pl->s2 = s2 ? 1 : 0;
   a.mchunks = a.pair ? a.Ma / 64 : a.Ma / 128; a.nchunks = a.Nb / BN; a.taps = ksize * ksize; a.ksize = ksize;
   a.tw = pow2_tile_w(W, WG_KT); a.th = pow2_tile_w(H, WG_KT / a.tw); a.tn = WG_KT / (a.tw * a.th);
   a.tiles_x = W / a.tw; a.tiles_y = H / a.th; a.tiles_b = (B + a.tn - 1) / a.tn;
@@ -336,13 +382,26 @@ static int wgrad_create(pdae_wgrad_tc_plan** plan_out, const void* act, const vo
   const int Ca = (split ? 3 : 1) * a.Ma, Cb = (split ? 3 : 1) * a.Nb;
   cuuint32_t estr4[4] = {1, 1, 1, 1};
   cuuint32_t box[4] = {64, (cuuint32_t)a.tw, (cuuint32_t)a.th, (cuuint32_t)a.tn};
+  cuuint32_t estr5[5] = {1, 1, 1, 1, 1};
+  cuuint32_t box5[5] = {64, (cuuint32_t)a.tw, 1, (cuuint32_t)a.th, (cuuint32_t)a.tn};
   for (int i = 0; i < 2; ++i) {
     const int C = i ? Cb : Ca;
-    cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
-    cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
-    CUresult r = enc(i ? &pl->tmB : &pl->tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(i ? Bt : At), dims, strides, box,
-                     estr4, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
-                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    CUresult r;
+    if (s2 && (i == 0) == (a.a_is_act == 1)) {
+      // the activation's parity view [B][Ha/2][2][Wa/2][2C] (conv_tc2.cu)
+      const cuuint64_t c2 = 2ull * C;
+      cuuint64_t dims[5] = {c2, (cuuint64_t)Wa / 2, 2, (cuuint64_t)Ha / 2, (cuuint64_t)B};
+      cuuint64_t strides[4] = {c2 * 2, (cuuint64_t)Wa * C * 2, 2ull * Wa * C * 2, (cuuint64_t)Ha * Wa * C * 2};
+      r = enc(i ? &pl->tmB : &pl->tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 5, const_cast<void*>(i ? Bt : At), dims, strides, box5, estr5,
+              CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    } else {
+      cuuint64_t dims[4] = {(cuuint64_t)C, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
+      cuuint64_t strides[3] = {(cuuint64_t)C * 2, (cuuint64_t)W * C * 2, (cuuint64_t)H * W * C * 2};
+      r = enc(i ? &pl->tmB : &pl->tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 4, const_cast<void*>(i ? Bt : At), dims, strides, box,
+              estr4, CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+              CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    }
     if (r != CUDA_SUCCESS) {
       delete pl;
       set_error("wgrad_tc_create: cuTensorMapEncodeTiled failed with %d", (int)r);
@@ -363,11 +422,19 @@ extern "C" int pdae_wgrad_tc_create_bf16(pdae_wgrad_tc_plan** plan_out, const vo
   return wgrad_create(plan_out, act_bf16, dy_bf16, dw, B, H, W, Cin, Cout, ksize, false);
 }
 
+extern "C" int pdae_wgrad_tc_create_bf16_s2(pdae_wgrad_tc_plan** plan_out, const void* act_bf16, const void* dy_bf16, float* dw,
+                                            int B, int H, int W, int Cin, int Cout) {
+  return wgrad_create(plan_out, act_bf16, dy_bf16, dw, B, H, W, Cin, Cout, 3, false, true);
+}
+
 extern "C" int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* pl, pdae_stream_t stream) {
   PDAE_REQUIRE(pl, "wgrad_tc_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
-  if (pl->split)
+  if (pl->s2)
+    e = pl->BN == 128 ? launch_wg<128, false, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s)
+                      : launch_wg<64, false, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s);
+  else if (pl->split)
     e = pl->BN == 128 ? launch_wg<128, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s)
                       : launch_wg<64, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s);
   else

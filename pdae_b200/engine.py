@@ -311,6 +311,9 @@ class Plan:
             if fn in ("wgrad_tc", "wgrad_tc_bf16"):
                 compiled.append(self._compile_wgrad(args, split=fn == "wgrad_tc"))
                 continue
+            if fn in ("conv_tc2_s2", "conv_tc2_s2_dgrad", "wgrad_tc_bf16_s2"):
+                compiled.append(self._compile_s2(fn, args))
+                continue
             cargs = []
             sidx = -1
             for k, a in enumerate(args):
@@ -392,6 +395,26 @@ class Plan:
         _native.check(rc, create.__name__)
         self._wg_handles.append(h)
         return (self.L.pdae_wgrad_tc_run, [h, None], 1, "wgrad_tc" if split else "wgrad_tc_bf16")
+
+    def _compile_s2(self, fn, args):
+        """3x3 stride-2 convs of a bf16 training step: forward (a = bf16 input, b = [9][Cout][Cin] weights, c = fp32 output),
+        data gradient (a = bf16 dy, b = [9][Cin][Cout] weights, c = fp32 dx), weight gradient (a = bf16 input, b = bf16 dy,
+        c = fp32 dw).  H, W: the conv's input size."""
+        h = ctypes.c_void_p()
+        if fn == "conv_tc2_s2":
+            a, b, bias, c, B, H, W, Cin, Cout = args
+            create, extra = self.L.pdae_conv_tc2_create_s2, [self._resolve(bias)]
+        else:
+            a, b, c, B, H, W, Cin, Cout = args
+            create = self.L.pdae_conv_tc2_create_s2_dgrad if fn == "conv_tc2_s2_dgrad" else self.L.pdae_wgrad_tc_create_bf16_s2
+            extra = []
+        rc = create(ctypes.byref(h), self._resolve(a), self._resolve(b), *extra, self._resolve(c), B, H, W, Cin, Cout)
+        _native.check(rc, create.__name__)
+        if fn == "wgrad_tc_bf16_s2":
+            self._wg_handles.append(h)
+            return (self.L.pdae_wgrad_tc_run, [h, None], 1, fn)
+        self._tc2_handles.append(h)
+        return (self.L.pdae_conv_tc2_run, [h, None], 1, fn)
 
     def _compile_gemm_softmax(self, args):
         a, a_ld, a_bs, b, b_ld, b_bs, out, o_ld, o_bs, batch, M, N, K, alpha = args
@@ -565,6 +588,20 @@ class Plan:
         with (e.g. the transposed, flipped weights of a dgrad) -- the packed copy still tracks the PARAMETER's version.
         Returns the per-channel (sum, sum^2) buffer [B][Cout][2] if the tensor-core epilogue produced one."""
         pad = k // 2 if pad is None else pad
+        if (self.train_tc == "bf16" and stride == 2 and k == 3 and pad == 1 and x.dtype == torch.float32
+                and out.dtype == torch.float32 and not (in_nchw or out_nchw or a_silu) and skip is None and w_transform is None
+                and residual is None and self.L.pdae_conv_s2_tc_supported(H, W, Cin, Cout)):
+            # 3x3 stride-2 conv of a bf16 training forward (the semantic encoder under autocast): conv_tc2 reads a plain bf16
+            # copy of the input through its parity view; the backward's weight gradient reads the same copy
+            xt = self.new((B, H, W, Cin), torch.bfloat16, "train_bf16")
+            self.call("gn_apply", x, PDAE_F32, Cin, None, PDAE_F32, 0, None, 0, RESAMPLE_NONE, B, H, W, xt, PDAE_BF16, None,
+                      PDAE_F32, _STREAM)
+            wp = self.pack((wkey or id(weight), "tc"), [weight],
+                           lambda: weight.detach().reshape(Cout, Cin, 9).permute(2, 0, 1).to(torch.bfloat16))
+            x.tc_copy = xt
+            self.call("conv_tc2_s2", xt, wp, self.param(bias), out, B, H, W, Cin, Cout,
+                      flops=2.0 * B * (H // 2) * (W // 2) * Cout * Cin * 9)
+            return None
         if (self.train_tc and x.dtype == torch.float32 and out.dtype == torch.float32 and not (in_nchw or out_nchw or a_silu)
                 and skip is None and w_transform is None and pad == k // 2 and self._tc_shape_ok(Cin, Cout, k, stride, H, W)):
             if self.train_tc == "bf16x3":

@@ -16,7 +16,10 @@ Mixed precision: a ShiftUNet / UNet training forward called inside ``torch.autoc
 ``enable_amp``; either autocast dtype) builds separate bf16 trainers: the frozen half runs as a plain "bf16" plan, and the
 forward convs, data gradients and weight gradients of the trainable convs are single-pass bf16 MMAs with fp32 accumulation.
 Activations, GroupNorm, attention and every gradient stay fp32, so the reference's ``GradScaler`` works unchanged.  The
-encoder and the latent MLP ignore autocast.
+semantic encoder does the same: under autocast its stride-2 convs (forward, data and weight gradient through parity views,
+``pdae_conv_tc2_create_s2*``, ``pdae_wgrad_tc_create_bf16_s2``) and its attention 1x1 convs are single-pass bf16 MMAs; its
+3-channel stem and final Linear stay fp32 on CUDA cores.  The latent MLP ignores autocast, and so does every forward-only
+call (sampling, ``infer_latents``, a frozen encoder).
 """
 from __future__ import annotations
 
@@ -149,12 +152,26 @@ class Backward:
         Ho, Wo = (H + 2 * pad - k) // stride + 1, (W + 2 * pad - k) // stride + 1
         kk = k * k
         same = stride == 1 and k in (1, 3) and pad == k // 2 and not in_nchw
+        # 3x3 stride-2 conv in the "bf16" backward (the semantic encoder under autocast): data and weight gradient on the
+        # tensor cores through parity views (conv_tc2.cu, wgrad_tc.cu), fed by one bf16 copy of dy
+        s2 = (P.precision == "bf16" and stride == 2 and k == 3 and pad == 1 and not (in_nchw or a_silu)
+              and bool(P.L.pdae_conv_s2_tc_supported(H, W, Cin, Cout)))
         # tensor-core operands: split [hi | lo | hi] blocks in the "bf16x3" backward, plain bf16 in the "bf16" (autocast) one
         ce = 3 if P.x3 else 1
         dy3 = None
         if trainable:
             dw = P.new_zeroed(kk * Cin * Cout)
-            if same and not a_silu and P.L.pdae_wgrad_tc_supported(H, W, Cin, Cout, k):
+            if s2:
+                act = getattr(x, "tc_copy", None)     # left by the bf16 training forward (Plan.conv)
+                if act is not None and tuple(act.shape) == (B, H, W, Cin):
+                    act = self.fx(act)
+                else:
+                    act, _ = P.gn_apply(self.fx(x), Cin, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=H, W=W,
+                                        act_dtype=torch.bfloat16)
+                dy3, _ = P.gn_apply(dy, Cout, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=Ho, W=Wo,
+                                    act_dtype=torch.bfloat16)
+                P.call("wgrad_tc_bf16_s2", act, dy3, dw, B, H, W, Cin, Cout, flops=2.0 * B * Ho * Wo * Cin * Cout * kk)
+            elif same and not a_silu and P.L.pdae_wgrad_tc_supported(H, W, Cin, Cout, k):
                 # weight gradient on the tensor cores (wgrad_tc.cu): fp32-grade split products, or single-pass bf16
                 a3 = getattr(x, "tc_copy", None)       # left by the tensor-core training forward (Plan.conv, train_tc)
                 if a3 is not None and tuple(a3.shape) == (B, H, W, ce * Cin):
@@ -177,6 +194,16 @@ class Backward:
                 self.sink.add(bias, db, Cout, lambda t: t)
         if not need_dx:
             return None
+        if s2:
+            # sub-pixel phases of dx, each a stride-1 correlation of dy with 1, 2, 2 or 4 taps of the transposed weights
+            if dy3 is None:
+                dy3, _ = P.gn_apply(dy, Cout, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=Ho, W=Wo,
+                                    act_dtype=torch.bfloat16)
+            wt = P.pack((id(weight), "tc_s2_dgrad"), [weight],
+                        lambda: weight.detach().reshape(Cout, Cin, kk).permute(2, 1, 0).to(torch.bfloat16))
+            dx = P.new((B, H, W, Cin), torch.float32, "dx")
+            P.call("conv_tc2_s2_dgrad", dy3, wt, dx, B, H, W, Cin, Cout, flops=2.0 * B * Ho * Wo * Cin * Cout * kk)
+            return dx
         if same and P.use_tc(Cout, Cin, k, 1, H, W):
             # dgrad of a stride-1 "same" conv = conv of dy with the transposed, spatially flipped weights: on the tensor
             # cores in the split-operand (fp32-grade) mode -- dy is split [hi | lo | hi], W' packed [W'_hi | W'_hi | W'_lo] --
@@ -633,11 +660,18 @@ def unet_train_forward(net, x, t, cond):
 # Semantic encoder
 # ======================================================================================================================
 class EncoderTrainer(_Generation):
-    def __init__(self, enc, B: int, H: int, W: int):
+    """Forward (fp32, all intermediates kept) + backward plans of a semantic encoder for one input shape; `amp`: the bf16
+    plans of a forward under autocast -- its stride-2 and attention convs, their data and weight gradients run as single-pass
+    bf16 MMAs (the 3-channel stem and the final Linear stay on CUDA cores)."""
+
+    def __init__(self, enc, B: int, H: int, W: int, amp: bool = False):
         self.enc = enc
+        self.amp = amp
         dev = enc._device()
         P = Plan(dev, "fp32")
         P.keep_all = True
+        if amp:
+            P.train_tc = "bf16"
         self.x_in = P.new((B, 3, H, W), torch.float32, "x_nchw")
         tape = []          # ("conv", mod, dict) / ("attn", ...) / ("fc", ...)
         h: Optional[Src] = None
@@ -676,7 +710,7 @@ class EncoderTrainer(_Generation):
         P.finalize()
         self.fwd = P
 
-        BP = bwd_plan(dev)
+        BP = bwd_plan(dev, amp)
         self.sink = GradSink()
         bw = Backward(BP, self.sink)
         L = enc.latent_dim
@@ -746,10 +780,12 @@ class _EncoderFn(torch.autograd.Function):
 def encoder_train_forward(enc, x):
     B, C, H, W = x.shape
     cache = enc.__dict__.setdefault("_train_cache", {})
-    tr = cache.get((B, H, W))
+    amp = autocast_active()
+    key = (B, H, W, amp)
+    tr = cache.get(key)
     if tr is None or tr.fwd.stale() or tr.bwd.stale():
-        tr = EncoderTrainer(enc, B, H, W)
-        cache[(B, H, W)] = tr
+        tr = EncoderTrainer(enc, B, H, W, amp)
+        cache[key] = tr
     return _EncoderFn.apply(tr, x, *tr.params)
 
 

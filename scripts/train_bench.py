@@ -7,7 +7,8 @@ all-reduce + fused Adam/EMA step on the celeba64-proxy decoder + encoder.
 Arithmetic: decoder forward, data gradients (conv_tc2) and weight gradients (wgrad_tc) on the tensor cores in the
 split-operand fp32-grade mode; encoder and the stride-2 / 3-channel convs in fp32 on CUDA cores (DESIGN.md).  --amp bf16: the step
 runs inside torch.autocast("cuda", dtype=torch.bfloat16) (the reference's enable_amp), so the decoder trains on the bf16
-plans: frozen half in the "bf16" mode, single-pass bf16 forward convs, data and weight gradients.  --overlap 1: the decoder bucket's NCCL all-reduce is launched from a
+plans: frozen half in the "bf16" mode, single-pass bf16 forward convs, data and weight gradients; so does the encoder's
+stride-2 and attention convs (its 3-channel stem and final Linear stay fp32 on CUDA cores).  --overlap 1: the decoder bucket's NCCL all-reduce is launched from a
 post-accumulate-grad hook as soon as the ShiftUNet backward has delivered its gradients and runs while the encoder
 backward computes (pdae_b200.utils.dist.OverlappedGradAllReduce); --overlap 0: all-reduce after backward.
 Rank 0 prints one JSON line."""
@@ -103,8 +104,9 @@ if rank == 0:
         res["amp"] = args.amp
         res["config"] = ("celeba64-proxy encoder + ShiftUNet (shift half trainable), dropout 0.1, fused Adam+EMA, bf16 autocast; "
                          "frozen decoder half in bf16, trainable decoder forward, data and weight gradients as single-pass "
-                         "bf16 MMAs on the tensor cores; fp32 activations, GroupNorm and attention backward; encoder and "
-                         "stride-2 / 3-channel convs on CUDA cores (fp32)")
+                         "bf16 MMAs on the tensor cores, and so are the encoder's stride-2 and attention convs; fp32 "
+                         "activations, GroupNorm and attention backward; 3-channel convs and the encoder's Linear on CUDA "
+                         "cores (fp32)")
     print(json.dumps(res))
 if world > 1:
     dist.destroy_process_group()

@@ -1,5 +1,7 @@
 """Per-kernel device time of one PDAE training step's plans (frozen-half forward, trainable forward, backward, encoder fwd/bwd).
-usage: python scripts/train_profile.py [batch]"""
+usage: python scripts/train_profile.py [batch] [--amp {off,bf16}]
+--amp bf16: the step runs inside torch.autocast("cuda", dtype=torch.bfloat16), so the bf16 training plans are profiled."""
+import argparse
 import os
 import sys
 
@@ -12,7 +14,19 @@ from pdae_b200.model.representation_learning.encoder import CELEBA64Encoder
 from pdae_b200.model.shift_unet import ShiftUNet
 from pdae_b200.utils.synth import fill_module_, synth_images
 
-B = int(sys.argv[1]) if len(sys.argv) > 1 else 32
+ap = argparse.ArgumentParser()
+ap.add_argument("batch", type=int, nargs="?", default=32)
+ap.add_argument("--amp", choices=("off", "bf16"), default="off")
+args = ap.parse_args()
+B = args.batch
+
+
+def train_loss():
+    with torch.autocast("cuda", dtype=torch.bfloat16, enabled=args.amp == "bf16"):
+        return gd.representation_learning_train_one_batch(enc, dec, x0)["prediction_loss"]
+
+
+
 cfg, size = WORKLOADS["celeba64"][0], WORKLOADS["celeba64"][1]
 dev = torch.device("cuda")
 dec = fill_module_(ShiftUNet(latent_dim=512, **dict(cfg, dropout=0.1)), seed=0).to(dev)
@@ -22,8 +36,9 @@ dec.set_train_mode()
 dec.precision = enc.precision = "fp32"
 gd = GaussianDiffusion({"timesteps": 1000, "betas_type": "linear"}, dev)
 x0 = synth_images(B, 3, size, 3).to(dev)
+print(f"{torch.cuda.get_device_properties(dev).name}, batch {B}, amp {args.amp}")
 for _ in range(2):
-    loss = gd.representation_learning_train_one_batch(enc, dec, x0)["prediction_loss"]
+    loss = train_loss()
     loss.backward()
 tr = list(dec._train_cache.values())[0]
 te = list(enc._train_cache.values())[0]
@@ -56,7 +71,7 @@ for it in range(N + 2):
     torch.cuda.synchronize()
     h = [time.perf_counter()]
     ev[0].record()
-    loss = gd.representation_learning_train_one_batch(enc, dec, x0)["prediction_loss"]
+    loss = train_loss()
     ev[1].record(); h.append(time.perf_counter())
     loss.backward()
     ev[2].record(); h.append(time.perf_counter())
