@@ -253,6 +253,20 @@ int pdae_gemm_tc2_create(pdae_conv_tc2_plan** plan, const void* a_bf16, long lon
 int pdae_gemm_tc2_softmax_create(pdae_conv_tc2_plan** plan, const void* a_bf16, long long a_ld, long long a_bs,
                                  const void* b_bf16, long long b_ld, long long b_bs, void* out_bf16, long long out_ld,
                                  long long out_bs, int batch, int M, int N, int K, float alpha);
+/* Attention backward under autocast (bf16 operands, fp32 accumulation).  Batched GEMM with per-operand majors: out_i[M x N]
+ * (fp32) = A_i * B_i^T, where a_mn / b_mn = 0 means A_i is stored [M][K] / B_i [N][K] (K-major, as above) and 1 means A_i is
+ * stored [K][M] / B_i [K][N] (MN-major); *_ld = elements between consecutive stored rows, *_bs = between batch items
+ * (multiples of 8).  M % 128 == 0, N % 64 == 0, K % 64 == 0.  All arguments are checked before any CUDA call.              */
+int pdae_gemm_tc2_create_major(pdae_conv_tc2_plan** plan, const void* a_bf16, int a_mn, long long a_ld, long long a_bs,
+                               const void* b_bf16, int b_mn, long long b_ld, long long b_bs, float* out, long long out_ld,
+                               long long out_bs, int batch, int M, int N, int K);
+/* Softmax gradient: dS_i = alpha * P_i * (dP_i - rowsum(P_i * dP_i)) stored as bf16, with dP_i = dO_i * V_i^T (both K-major)
+ * accumulated in fp32 and consumed in the GEMM epilogue; P_i (bf16) has the output's [M][N] shape with strides p_ld / p_bs.
+ * N in {64, 128, 256}, alpha > 0, other bounds as above.  Run / destroy: pdae_conv_tc2_run / pdae_conv_tc2_destroy.           */
+int pdae_gemm_tc2_softmax_grad_create(pdae_conv_tc2_plan** plan, const void* do_bf16, long long a_ld, long long a_bs,
+                                      const void* v_bf16, long long b_ld, long long b_bs, const void* p_bf16, long long p_ld,
+                                      long long p_bs, void* ds_bf16, long long out_ld, long long out_bs, int batch, int M, int N,
+                                      int K, float alpha);
 /* 3x3, stride-2, pad-1 convs on plain bf16 operands with fp32 accumulation (the semantic encoder's training step under
  * autocast, model/representation_learning/encoder).  H, W: the conv's input size, both even; Cin % 64 == 0, Cout % 64 == 0
  * (pdae_conv_s2_tc_supported).  Forward: out[B][H/2][W/2][Cout] fp32 = conv(in[B][H][W][Cin] bf16, w[9][Cout][Cin] bf16)

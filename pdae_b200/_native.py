@@ -98,6 +98,10 @@ _SIGS = {
                                      c_int, c_int, c_int, c_int]),
     "pdae_gemm_tc2_softmax_create": (c_int, [POINTER(c_void_p), _P, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int64, c_int64,
                                              c_int, c_int, c_int, c_int, c_float]),
+    "pdae_gemm_tc2_create_major": (c_int, [POINTER(c_void_p), _P, c_int, c_int64, c_int64, _P, c_int, c_int64, c_int64, _P,
+                                           c_int64, c_int64, c_int, c_int, c_int, c_int]),
+    "pdae_gemm_tc2_softmax_grad_create": (c_int, [POINTER(c_void_p), _P, c_int64, c_int64, _P, c_int64, c_int64, _P, c_int64,
+                                                  c_int64, _P, c_int64, c_int64, c_int, c_int, c_int, c_int, c_float]),
     "pdae_conv_s2_tc_supported": (c_int, [c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_s2": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_s2_dgrad": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),

@@ -21,6 +21,15 @@
 //           ky = 1 (py = 0) or ky = 0 at dY row + 1 and ky = 2 at dY row + 0 (py = 1), likewise kx: 1, 2, 2 or 4 taps, 9 over
 //           the four phases (the forward's MMA count).  The phase is the fastest tile index, so every CTA's contiguous tile
 //           range mixes the cheap and the expensive phases; each tile is stored through the parity view of dX.
+//
+// GM != 0: batched-GEMM modes of the attention backward (bf16 autocast training).  GM_A_MN / GM_B_MN: the A / B operand is
+// MN-major, stored [K][M] / [K][N] with a row stride; each 64-wide MN block of a stage is one TMA box [64 k][64 mn] with
+// SWIZZLE_128B (wgmma.cuh: the MN-major SW128 atom stack wgrad_tc also reads).  GM_SMGRAD: the softmax-gradient epilogue; the
+// tile's accumulators hold dP = dO V^T for whole rows (N == BN), and the stored bf16 tile is
+//   dS = alpha * P * (dP - rowsum(P * dP)),
+// with P (bf16, the forward's probabilities) read for the same rows and columns, so dP never leaves the registers.  A 256-wide
+// row does not fit one warpgroup's registers beside the epilogue: with GM_SPLITN the tile is 64 rows x 2 BN columns, both
+// warpgroups reading the same A rows, warpgroup g computing columns [g BN, g BN + BN); the row sums meet in shared memory.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -35,6 +44,7 @@ constexpr int T2_STG_BYTES = 128 * 128;        // staging tile: 128 rows x 128 B
 constexpr int T2_MAX_STAGES = 8;
 constexpr int T2_THREADS = 288;   // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int T2_CONSUMERS = 256;
+constexpr int GM_A_MN = 1, GM_B_MN = 2, GM_SMGRAD = 4, GM_SPLITN = 8;   // conv_tc2_kernel's GM bits (kernel header)
 
 struct ConvTc2Args {
   const float* bias;
@@ -54,6 +64,12 @@ struct ConvTc2Args {
                   // region and reused by all of the CTA's tiles; pipeline stages then hold A tiles only
   float softmax_alpha;  // > 0: the epilogue stores softmax_row(alpha * acc) (bf16) instead of acc -- attention scores whose
                         // whole row lives in this tile's accumulators (N == BN); model/module.py:452-455,483-486
+};
+// GM_SMGRAD operands (a kernel parameter of its own: ConvTc2Args keeps its size, so the other modes compile as before)
+struct SmGradArgs {
+  const __nv_bfloat16* p;  // the probabilities P, indexed like the output: row stride ld, batch stride bs
+  long long ld, bs;
+  float alpha;             // the score scale folded into dS
 };
 
 __device__ __forceinline__ uint32_t s_u32(const void* p) { return (uint32_t)__cvta_generic_to_shared(p); }
@@ -144,19 +160,20 @@ __device__ __forceinline__ void cons_bar() { asm volatile("bar.sync 1, 256;" :::
 // byte offset of (row, 16-byte chunk) inside a 128-row x 128-byte SWIZZLE_128B staging tile
 __device__ __forceinline__ uint32_t swz(int row, int chunk16) { return (uint32_t)(row * 128 + ((chunk16 ^ (row & 7)) << 4)); }
 
-template <int BN, bool OB, int S2 = 0>
+template <int BN, bool OB, int S2 = 0, int GM = 0>
 __global__ void __launch_bounds__(T2_THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
                 const __grid_constant__ CUtensorMap tmA2, const __grid_constant__ CUtensorMap tmB2,
-                const __grid_constant__ CUtensorMap tmA3, ConvTc2Args p) {
+                const __grid_constant__ CUtensorMap tmA3, ConvTc2Args p, SmGradArgs sg) {
   extern __shared__ uint8_t smem_raw[];
   __shared__ __align__(8) uint64_t bar_full[T2_MAX_STAGES], bar_empty[T2_MAX_STAGES];
   __shared__ __align__(8) uint64_t bar_res, bar_w;
   __shared__ float st_acc[2][BN < 32 ? 32 : BN];  // [sum | sum^2][channel] of the current (image, n-tile)
   __shared__ float st_part[2][8][32];              // per-chunk partial sums [sum | sum^2][row run][column] (CW * 8 runs / 32)
 
-  constexpr int B_BYTES = BN * T2_BK * 2;
+  constexpr bool SPN = (GM & GM_SPLITN) != 0;   // 64-row tiles, the B tile holds 2 BN rows (one BN-row half per warpgroup)
+  constexpr int B_BYTES = (SPN ? 2 : 1) * BN * T2_BK * 2;
   constexpr int STAGE_BYTES = T2_A_BYTES + ((B_BYTES + 1023) / 1024) * 1024;
   constexpr int CW = OB ? 64 : 32;             // accumulator columns per staging tile (128-byte rows)
   constexpr int NCH = BN < CW ? 1 : BN / CW;
@@ -199,7 +216,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     int s = 0;
     uint32_t ph = 0;
     const bool ws = p.w_stat != 0;
-    const uint32_t stage_tx = ws ? (uint32_t)T2_A_BYTES : (uint32_t)(T2_A_BYTES + B_BYTES);
+    const uint32_t stage_tx = ws ? (uint32_t)T2_A_BYTES : (uint32_t)((SPN ? T2_A_BYTES / 2 : T2_A_BYTES) + B_BYTES);
     if (ws && tile_begin < tile_end) {   // all B tiles of the layer, once (single n-tile: n0 = 0)
       const uint32_t wb = s_u32(&bar_w);
       if (elect_one()) {
@@ -257,8 +274,22 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
         if (elect_one()) {
           mb_expect_tx(full, stage_tx);
-          tma_ld4(sa, &tmA, full, kb * T2_BK, x0 + dx, y0 + dy, b0);
-          if (!ws) tma_ld3(sa + T2_A_BYTES, &tmB, full, kb * T2_BK, n0, p.w_batched ? b0 : tap);
+          if constexpr ((GM & GM_A_MN) != 0) {        // [K][M] operand: one [64 k][64 m] box per consumer warpgroup
+            tma_ld3(sa, &tmA, full, x0, kb * T2_BK, b0);
+            tma_ld3(sa + wgmma::MN_BOX, &tmA, full, x0 + 64, kb * T2_BK, b0);
+          } else {
+            tma_ld4(sa, &tmA, full, kb * T2_BK, x0 + dx, y0 + dy, b0);
+          }
+          if constexpr ((GM & GM_B_MN) != 0) {        // [K][N] operand: BN / 64 boxes [64 k][64 n]
+#pragma unroll
+            for (int j = 0; j < BN / 64; ++j)
+              tma_ld3(sa + T2_A_BYTES + (uint32_t)j * wgmma::MN_BOX, &tmB, full, n0 + 64 * j, kb * T2_BK, b0);
+          } else if constexpr (SPN) {                 // both BN-row halves of the 2 BN-wide tile
+            tma_ld3(sa + T2_A_BYTES, &tmB, full, kb * T2_BK, n0, b0);
+            tma_ld3(sa + T2_A_BYTES + BN * T2_BK * 2, &tmB, full, kb * T2_BK, n0 + BN, b0);
+          } else {
+            if (!ws) tma_ld3(sa + T2_A_BYTES, &tmB, full, kb * T2_BK, n0, p.w_batched ? b0 : tap);
+          }
         }
         __syncwarp();
         if (++kb == p.kblocks) {
@@ -320,12 +351,26 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int it = 0; it < n_it; ++it) {
         mb_wait(s_u32(&bar_full[s]), ph);
         const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
-        const uint64_t ad = wgmma::desc_sw128(sa + (uint32_t)wg * (64u * 128u), 16u, 1024u);
-        const uint64_t bd = wgmma::desc_sw128(p.w_stat ? wbase + (uint32_t)(it * B_BYTES) : sa + T2_A_BYTES, 16u, 1024u);
-        wgmma::fence();
+        if constexpr (GM == 0) {
+          const uint64_t ad = wgmma::desc_sw128(sa + (uint32_t)wg * (64u * 128u), 16u, 1024u);
+          const uint64_t bd = wgmma::desc_sw128(p.w_stat ? wbase + (uint32_t)(it * B_BYTES) : sa + T2_A_BYTES, 16u, 1024u);
+          wgmma::fence();
 #pragma unroll
-        for (int k = 0; k < T2_BK / 16; ++k)
-          wgmma::mma<BN, 0>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (uint32_t)((it | k) != 0));
+          for (int k = 0; k < T2_BK / 16; ++k)
+            wgmma::mma<BN, 0>(acc, ad + (uint64_t)(2 * k), bd + (uint64_t)(2 * k), (uint32_t)((it | k) != 0));
+        } else {
+          constexpr int TA = (GM & GM_A_MN) ? 1 : 0, TB = (GM & GM_B_MN) ? 1 : 0;
+          constexpr uint64_t SA = TA ? wgmma::K16_STEP_MNMAJOR : wgmma::K16_STEP_KMAJOR;
+          constexpr uint64_t SB = TB ? wgmma::K16_STEP_MNMAJOR : wgmma::K16_STEP_KMAJOR;
+          const uint32_t a_s = SPN ? sa : sa + (uint32_t)wg * wgmma::MN_BOX;
+          const uint32_t b_s = sa + T2_A_BYTES + (SPN ? (uint32_t)(wg * BN * T2_BK * 2) : 0u);
+          const uint64_t ad = TA ? wgmma::desc_mnmajor(a_s) : wgmma::desc_kmajor(a_s);
+          const uint64_t bd = TB ? wgmma::desc_mnmajor(b_s) : wgmma::desc_kmajor(b_s);
+          wgmma::fence();
+#pragma unroll
+          for (int k = 0; k < T2_BK / 16; ++k)
+            wgmma::mma<BN, TA, TB>(acc, ad + (uint64_t)k * SA, bd + (uint64_t)k * SB, (uint32_t)((it | k) != 0));
+        }
         wgmma::commit();
         wgmma::wait<1>();
         if (prev >= 0 && lane == 0) mb_arrive(s_u32(&bar_empty[prev]));
@@ -375,7 +420,50 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           }
         }
       } else {
-        if (p.softmax_alpha > 0.f) {
+        // softmax-gradient epilogue (GM_SMGRAD): the thread's two rows (i / 2 % 2) are spread over the 4 lanes of a quad; P is
+        // read for exactly the (row, column pair)s its fragments hold.  rowsum(P dP) first, then dS chunk by chunk below.
+        constexpr bool SMG = (GM & GM_SMGRAD) != 0;
+        const __nv_bfloat16* sg_row =
+            SMG ? sg.p + (long long)b0 * sg.bs + (long long)(x0 + (SPN ? 0 : 64 * wg) + wgmma::frag_row(t, 0)) * sg.ld +
+                      (SPN ? wg * BN : 0)
+                : nullptr;
+        auto ld_p = [&](int i) -> uint32_t {     // P at the columns of fragment registers i, i + 1
+          return __ldg(reinterpret_cast<const unsigned int*>(sg_row + ((i >> 1) & 1) * 8 * sg.ld + wgmma::frag_col(t, i)));
+        };
+        float rs[2] = {0.f, 0.f};
+        if constexpr (SMG) {
+#pragma unroll
+          for (int c = 0; c < NCH; ++c) {
+            // (the empty asm keeps each chunk's loads behind the previous chunk's: the accumulators of a 256-wide row leave
+            //  room for one chunk of P words, not for all of them)
+            asm volatile("" ::: "memory");
+#pragma unroll
+            for (int i = c * (CW / 2); i < (c + 1) * (CW / 2); i += 2) {
+              const uint32_t w = ld_p(i);
+              rs[(i >> 1) & 1] = fmaf(__uint_as_float(w << 16), acc[i],
+                                      fmaf(__uint_as_float(w & 0xffff0000u), acc[i + 1], rs[(i >> 1) & 1]));
+            }
+          }
+#pragma unroll
+          for (int h = 0; h < 2; ++h) {
+            rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 1);
+            rs[h] += __shfl_xor_sync(0xffffffffu, rs[h], 2);
+          }
+          if constexpr (SPN) {
+            // the other half of each row is in the other warpgroup: [warpgroup][row] partial sums, added in the same order by
+            // both.  (The next tile writes them again only after the chunk loop's barriers, which follow these reads.)
+            float* xs = &st_part[0][0][0];
+            const int fr = wgmma::frag_row(t, 0);
+            if ((t & 3) == 0) {
+              xs[64 * wg + fr] = rs[0];
+              xs[64 * wg + fr + 8] = rs[1];
+            }
+            cons_bar();
+            rs[0] = xs[fr] + xs[64 + fr];
+            rs[1] = xs[fr + 8] + xs[64 + fr + 8];
+          }
+        }
+        if (GM == 0 && p.softmax_alpha > 0.f) {
           // softmax epilogue: the thread's two rows (i / 2 % 2) are spread over the 4 lanes of a quad
           const float sm_a = p.softmax_alpha * 1.4426950408889634f;
           float mx[2] = {-3.0e38f, -3.0e38f}, sum[2] = {0.f, 0.f};
@@ -403,6 +491,15 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           float v[CW / 2];
 #pragma unroll
           for (int q = 0; q < CW / 2; ++q) v[q] = acc[c * (CW / 2) + q];
+          if constexpr (SMG) {                  // dS = alpha P (dP - rowsum(P dP))
+#pragma unroll
+            for (int q = 0; q < CW / 2; q += 2) {
+              const uint32_t w = ld_p(c * (CW / 2) + q);
+              const float r = rs[(q >> 1) & 1];
+              v[q] = sg.alpha * __uint_as_float(w << 16) * (v[q] - r);
+              v[q + 1] = sg.alpha * __uint_as_float(w & 0xffff0000u) * (v[q + 1] - r);
+            }
+          }
           if (p.bias) {
 #pragma unroll
             for (int q = 0; q < CW / 2; q += 2) {
@@ -454,7 +551,10 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
           cons_bar();
           if (elected) {
             if constexpr (S2 == 2) tma_st5(&tmO, obuf, (ph2 & 1) * p.Cout + n0 + c * CW, x0, ph2 >> 1, y0, b0);   // dX parity view
-            else tma_st4(&tmO, obuf, n0 + c * CW, x0, y0, b0);
+            else if constexpr (SPN) {       // staging rows [64 g, 64 g + 64) = warpgroup g's columns of the tile's 64 rows
+              tma_st4(&tmO, obuf, n0 + c * CW, x0, y0, b0);
+              tma_st4(&tmO, obuf + 64u * 128u, n0 + BN + c * CW, x0, y0, b0);
+            } else tma_st4(&tmO, obuf, n0 + c * CW, x0, y0, b0);
             asm volatile("cp.async.bulk.commit_group;" ::: "memory");
           }
           if (p.ch_stats) {
@@ -591,17 +691,17 @@ static int pow2_tile(int W, int cap) {
   return t;
 }
 
-template <int BN, bool OB, int S2 = 0>
+template <int BN, bool OB, int S2 = 0, int GM = 0>
 static cudaError_t launch_tc2(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r,
                               const CUtensorMap& a2, const CUtensorMap& b2, const CUtensorMap& a3, const ConvTc2Args& args,
-                              int grid, size_t smem, cudaStream_t s) {
+                              const SmGradArgs& sg, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, OB, S2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, stats <= 2 KB) <= 227 KB
+    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, OB, S2, GM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, stats <= 2 KB) <= 227 KB
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  conv_tc2_kernel<BN, OB, S2><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args);
+  conv_tc2_kernel<BN, OB, S2, GM><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args, sg);
   return cudaPeekAtLastError();
 }
 
@@ -612,8 +712,10 @@ using namespace pdae;
 struct pdae_conv_tc2_plan {
   CUtensorMap tmA, tmB, tmO, tmR, tmA2, tmB2, tmA3;
   ConvTc2Args args;
+  SmGradArgs sg;
   int BN, grid;
   int s2;           // 0: stride-1 conv / GEMM; 1: stride-2 forward; 2: stride-2 data gradient (conv_tc2_kernel's S2)
+  int gm;           // batched-GEMM operand / epilogue mode (conv_tc2_kernel's GM)
   size_t smem;
 };
 
@@ -633,6 +735,8 @@ struct Tc2Desc {
   const void* in3 = nullptr; int Cin2a = 0;   // skip input = channel concat of in2 [..,Cin2a] and in3 [..,Cin2-Cin2a] (in3 == nullptr: in2 alone)
   int s2 = 0;   // stride-2 3x3 conv (kernel header): H, W are the OUTPUT / dY grid; 1: `in` is read through its parity view;
                 // 2: data gradient, `out` (fp32 dX) is written through its parity view
+  int gm = 0;   // batched GEMM only: GM_A_MN / GM_B_MN operands ([K][M] / [K][N], in_ld / w_ld between k rows), GM_SMGRAD epilogue
+  const void* sg_p = nullptr; long long sg_ld = 0, sg_bs = 0; float sg_alpha = 0.f;   // GM_SMGRAD: P and alpha
 };
 
 static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
@@ -665,7 +769,9 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
   a.tw = pow2_tile(W, T2_BM);
   a.th = pow2_tile(H, T2_BM / a.tw);
   a.tn = T2_BM / (a.tw * a.th);
-  if (W % a.tw != 0 || H % a.th != 0 || a.tw * a.th * a.tn != T2_BM || a.tn > 256 || (d.w_batched && a.tn != 1)) {
+  const bool spn = (d.gm & GM_SPLITN) != 0;   // 64-row tiles (batched GEMM, H == 1)
+  if (spn) a.tw = 64;
+  if (W % a.tw != 0 || H % a.th != 0 || a.tw * a.th * a.tn != (spn ? 64 : T2_BM) || a.tn > 256 || (d.w_batched && a.tn != 1)) {
     delete pl;
     PDAE_REQUIRE(false, "conv_tc2_create: H=%d W=%d cannot be tiled into 128-pixel boxes%s", H, W,
                  d.w_batched ? " of a single image (batched GEMM)" : "");
@@ -692,10 +798,13 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
     delete pl;
     PDAE_REQUIRE(false, "conv_tc2_create: Cout=%d not a multiple of BN=%d", Cout, BN);
   }
+  if (spn) BN /= 2;   // per warpgroup
   pl->BN = BN;
   pl->s2 = d.s2;
-  a.tiles_total = a.tiles_m * (head ? 1 : Cout / BN) * (d.s2 == 2 ? 4 : 1);   // stride-2 dgrad: x 4 sub-pixel phases
-  const int b_bytes = ((BN * T2_BK * 2 + 1023) / 1024) * 1024;
+  pl->gm = d.gm;
+  pl->sg.p = static_cast<const __nv_bfloat16*>(d.sg_p); pl->sg.ld = d.sg_ld; pl->sg.bs = d.sg_bs; pl->sg.alpha = d.sg_alpha;
+  a.tiles_total = a.tiles_m * (head ? 1 : Cout / (spn ? 2 * BN : BN)) * (d.s2 == 2 ? 4 : 1);   // stride-2 dgrad: x 4 phases
+  const int b_bytes = ((BN * T2_BK * 2 + 1023) / 1024) * 1024 * (spn ? 2 : 1);
   int stage_bytes = T2_A_BYTES + b_bytes;
   const int staging = head ? 0 : (a.has_res ? 2 : 1) * T2_STG_BYTES;
   const int total_all = a.taps * a.kblocks + a.kblocks2;
@@ -738,6 +847,16 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
                      CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail("A (parity view)", (int)r);
+  } else if (d.gm & GM_A_MN) {
+    // [batch][K][M] with row stride in_ld: one [64 k][64 m] box per consumer warpgroup
+    cuuint64_t dims[3] = {(cuuint64_t)W, (cuuint64_t)Cin, (cuuint64_t)B};
+    cuuint64_t strides[2] = {(cuuint64_t)d.in_ld * 2, (cuuint64_t)d.in_bs * 2};
+    cuuint32_t box[3] = {64, (cuuint32_t)T2_BK, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(&pl->tmA, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d.in), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_128B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail("A (MN-major)", (int)r);
   } else {
     cuuint64_t dims[4] = {(cuuint64_t)Cin, (cuuint64_t)W, (cuuint64_t)H, (cuuint64_t)B};
     cuuint64_t strides[3] = {(cuuint64_t)d.in_ld * 2, (cuuint64_t)W * d.in_ld * 2, (cuuint64_t)d.in_bs * 2};
@@ -747,7 +866,17 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
                      CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
     if (r != CUDA_SUCCESS) return fail("A", (int)r);
   }
-  {
+  if (d.gm & GM_B_MN) {
+    // [batch][K][N] with row stride w_ld: BN / 64 boxes [64 k][64 n] per stage
+    cuuint64_t dims[3] = {(cuuint64_t)Cout, (cuuint64_t)Cin, (cuuint64_t)B};
+    cuuint64_t strides[2] = {(cuuint64_t)d.w_ld * 2, (cuuint64_t)d.w_bs * 2};
+    cuuint32_t box[3] = {64, (cuuint32_t)T2_BK, 1};
+    cuuint32_t estr[3] = {1, 1, 1};
+    CUresult r = enc(&pl->tmB, CU_TENSOR_MAP_DATA_TYPE_BFLOAT16, 3, const_cast<void*>(d.w), dims, strides, box, estr,
+                     CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+                     CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE);
+    if (r != CUDA_SUCCESS) return fail("W (MN-major)", (int)r);
+  } else {
     cuuint64_t dims[3] = {(cuuint64_t)Cin, (cuuint64_t)Cout, (cuuint64_t)(d.w_batched ? B : a.taps)};
     cuuint64_t strides[2] = {(cuuint64_t)d.w_ld * 2, (cuuint64_t)d.w_bs * 2};
     cuuint32_t box[3] = {(cuuint32_t)T2_BK, (cuuint32_t)BN, 1};
@@ -898,6 +1027,66 @@ extern "C" int pdae_gemm_tc2_softmax_create(pdae_conv_tc2_plan** plan_out, const
   return tc2_create(plan_out, d);
 }
 
+// ---- batched GEMMs of the attention backward (bf16 autocast training) ---------------------------------------------------
+// Every argument is checked before any CUDA call.
+static int gemm_validate(const char* fn, const void* a, const void* b, const void* out, long long a_ld, long long a_bs,
+                         long long b_ld, long long b_bs, long long out_ld, long long out_bs, int batch, int M, int N, int K) {
+  PDAE_REQUIRE(a && b && out, "%s: null pointer", fn);
+  PDAE_REQUIRE(!(((uintptr_t)a | (uintptr_t)b | (uintptr_t)out) & 15), "%s: pointers must be 16-byte aligned", fn);
+  PDAE_REQUIRE(!((a_ld | a_bs | b_ld | b_bs | out_ld | out_bs) & 7) && a_ld > 0 && b_ld > 0 && out_ld > 0 && a_bs >= 0 &&
+                   b_bs >= 0 && out_bs >= 0,
+               "%s: strides must be positive multiples of 16 bytes", fn);
+  PDAE_REQUIRE(batch > 0 && M > 0 && N > 0 && K > 0 && M % 128 == 0 && N % 64 == 0 && K % 64 == 0,
+               "%s: batch=%d M=%d N=%d K=%d: need M %% 128 == 0, N %% 64 == 0, K %% 64 == 0", fn, batch, M, N, K);
+  return PDAE_OK;
+}
+
+// out_i[M x N] (fp32) = A_i * B_i^T for every batch item i, each operand K-major (a_mn / b_mn = 0: A_i stored [M][K], B_i
+// [N][K]) or MN-major (1: A_i stored [K][M], B_i [K][N]); *_ld = elements between consecutive stored rows, *_bs = between items.
+extern "C" int pdae_gemm_tc2_create_major(pdae_conv_tc2_plan** plan_out, const void* a_bf16, int a_mn, long long a_ld,
+                                          long long a_bs, const void* b_bf16, int b_mn, long long b_ld, long long b_bs, float* out,
+                                          long long out_ld, long long out_bs, int batch, int M, int N, int K) {
+  static const char* fn = "gemm_tc2_create_major";
+  PDAE_REQUIRE(plan_out, "%s: null pointer", fn);
+  PDAE_REQUIRE((a_mn == 0 || a_mn == 1) && (b_mn == 0 || b_mn == 1), "%s: major flags must be 0 (K-major) or 1 (MN-major)", fn);
+  const int rc = gemm_validate(fn, a_bf16, b_bf16, out, a_ld, a_bs, b_ld, b_bs, out_ld, out_bs, batch, M, N, K);
+  if (rc != PDAE_OK) return rc;
+  Tc2Desc d;
+  d.in = a_bf16; d.w = b_bf16; d.bias = nullptr; d.residual = nullptr; d.out = out; d.out_dtype = PDAE_F32;
+  d.ch_stats = nullptr; d.B = batch; d.H = 1; d.W = M; d.Cin = K; d.Cout = N; d.ksize = 1; d.cout_valid = 0; d.bn_override = 0;
+  d.in_ld = a_ld; d.in_bs = a_bs;
+  d.w_batched = 1; d.w_ld = b_ld; d.w_bs = b_bs;
+  d.out_ld = out_ld; d.out_bs = out_bs;
+  d.gm = (a_mn ? GM_A_MN : 0) | (b_mn ? GM_B_MN : 0);
+  return tc2_create(plan_out, d);
+}
+
+// dS_i = alpha * P_i * (dP_i - rowsum(P_i * dP_i)) stored as bf16, dP_i = dO_i * V_i^T (both K-major, strides as in
+// pdae_gemm_tc2_create) computed in fp32 and consumed in the epilogue; P_i (bf16) has the output's shape, strides p_ld / p_bs.
+// N in {64, 128, 256}: one n-tile holds a whole row.
+extern "C" int pdae_gemm_tc2_softmax_grad_create(pdae_conv_tc2_plan** plan_out, const void* do_bf16, long long a_ld, long long a_bs,
+                                                 const void* v_bf16, long long b_ld, long long b_bs, const void* p_bf16,
+                                                 long long p_ld, long long p_bs, void* ds_bf16, long long out_ld, long long out_bs,
+                                                 int batch, int M, int N, int K, float alpha) {
+  static const char* fn = "gemm_tc2_softmax_grad_create";
+  PDAE_REQUIRE(plan_out && p_bf16, "%s: null pointer", fn);
+  PDAE_REQUIRE(!((uintptr_t)p_bf16 & 15), "%s: pointers must be 16-byte aligned", fn);
+  const int rc = gemm_validate(fn, do_bf16, v_bf16, ds_bf16, a_ld, a_bs, b_ld, b_bs, out_ld, out_bs, batch, M, N, K);
+  if (rc != PDAE_OK) return rc;
+  PDAE_REQUIRE(!((p_ld | p_bs) & 7) && p_ld > 0 && p_bs >= 0, "%s: strides must be positive multiples of 16 bytes", fn);
+  PDAE_REQUIRE(N == 64 || N == 128 || N == 256, "%s: N=%d must be 64, 128 or 256", fn, N);
+  PDAE_REQUIRE(alpha > 0.f, "%s: alpha must be positive", fn);
+  Tc2Desc d;
+  d.in = do_bf16; d.w = v_bf16; d.bias = nullptr; d.residual = nullptr; d.out = ds_bf16; d.out_dtype = PDAE_BF16;
+  d.ch_stats = nullptr; d.B = batch; d.H = 1; d.W = M; d.Cin = K; d.Cout = N; d.ksize = 1; d.cout_valid = 0; d.bn_override = N;
+  d.in_ld = a_ld; d.in_bs = a_bs;
+  d.w_batched = 1; d.w_ld = b_ld; d.w_bs = b_bs;
+  d.out_ld = out_ld; d.out_bs = out_bs;
+  d.gm = N == 256 ? GM_SMGRAD | GM_SPLITN : GM_SMGRAD;
+  d.sg_p = p_bf16; d.sg_ld = p_ld; d.sg_bs = p_bs; d.sg_alpha = alpha;
+  return tc2_create(plan_out, d);
+}
+
 // ---- 3x3, stride-2, pad-1 convs on plain bf16 operands (the semantic encoder's bf16 autocast training step) ----------------
 // H, W: the conv's INPUT size (even); the output / dY grid is H/2 x W/2.  Every tile shape the 128- and 64-pixel boxes of
 // conv_tc2 / wgrad_tc need exists for such a grid (power-of-two tiles, several images per box when the grid is small).
@@ -955,11 +1144,19 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
   PDAE_REQUIRE(pl, "conv_tc2_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
-#define T2_GO(BN, OB) launch_tc2<BN, OB>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s)
+#define T2_GO(BN, OB) launch_tc2<BN, OB>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
 #define T2_GO_S2(BN, S2) \
-  launch_tc2<BN, false, S2>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->grid, pl->smem, s)
+  launch_tc2<BN, false, S2>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
+#define T2_GO_GM(BN, OB, GM) \
+  launch_tc2<BN, OB, 0, GM>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
   const bool ob = pl->args.out_bf16 != 0;
-  if (pl->s2 == 1) e = pl->BN == 128 ? T2_GO_S2(128, 1) : T2_GO_S2(64, 1);
+  if (pl->gm == (GM_SMGRAD | GM_SPLITN)) e = T2_GO_GM(128, true, GM_SMGRAD | GM_SPLITN);
+  else if (pl->gm == GM_SMGRAD) e = pl->BN == 128 ? T2_GO_GM(128, true, GM_SMGRAD) : T2_GO_GM(64, true, GM_SMGRAD);
+  else if (pl->gm == GM_A_MN) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_A_MN) : T2_GO_GM(64, false, GM_A_MN);
+  else if (pl->gm == GM_B_MN) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_B_MN) : T2_GO_GM(64, false, GM_B_MN);
+  else if (pl->gm == (GM_A_MN | GM_B_MN))
+    e = pl->BN == 128 ? T2_GO_GM(128, false, GM_A_MN | GM_B_MN) : T2_GO_GM(64, false, GM_A_MN | GM_B_MN);
+  else if (pl->s2 == 1) e = pl->BN == 128 ? T2_GO_S2(128, 1) : T2_GO_S2(64, 1);
   else if (pl->s2 == 2) e = pl->BN == 128 ? T2_GO_S2(128, 2) : T2_GO_S2(64, 2);
   else switch (pl->BN) {
     case 16: e = T2_GO(16, false); break;
@@ -969,9 +1166,10 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
   }
 #undef T2_GO
 #undef T2_GO_S2
+#undef T2_GO_GM
   if (e != cudaSuccess) {
     (void)cudaGetLastError();
-    set_error("launch of conv_tc2_kernel<%d> failed: %s", pl->BN, cudaGetErrorString(e));
+    set_error("launch of conv_tc2_kernel<%d> (mode %d) failed: %s", pl->BN, pl->gm, cudaGetErrorString(e));
     return PDAE_ECUDA;
   }
   return PDAE_OK;

@@ -38,7 +38,7 @@
 namespace pdae {
 
 constexpr int WG_KT = 64;                 // pixels per k-tile (= rows of one TMA box)
-constexpr int WG_BOX = WG_KT * 128;       // bytes of one [64 px][64 ch] box
+constexpr int WG_BOX = wgmma::MN_BOX;     // bytes of one [64 px][64 ch] box (WG_KT rows of 128 B)
 constexpr int WG_THREADS = 288;
 constexpr int WG_MAX_ST = 4;              // stage ring depth cap of the split variant (its 48-64 KB stages fit 3-4)
 constexpr int WG_MAX_ST_BF16 = 8;         // plain bf16 variant: 24-32 KB stages, up to 8 in the same shared-memory budget
@@ -238,24 +238,24 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       mb_wait(s_u32(&bar_full[s]), ph);
       const uint32_t base = smem0 + (uint32_t)(s * STAGE) + (uint32_t)(wgi * WG_BOX);
       if constexpr (SPLIT) {
-        const uint64_t a_hi = wgmma::desc_sw128(base, WG_BOX, 1024u), a_lo = wgmma::desc_sw128(base + A_BYTES, WG_BOX, 1024u);
+        const uint64_t a_hi = wgmma::desc_mnmajor(base), a_lo = wgmma::desc_mnmajor(base + A_BYTES);
         const uint32_t bb = smem0 + (uint32_t)(s * STAGE) + 2u * A_BYTES;
-        const uint64_t b_hi = wgmma::desc_sw128(bb, WG_BOX, 1024u), b_lo = wgmma::desc_sw128(bb + B_BYTES, WG_BOX, 1024u);
+        const uint64_t b_hi = wgmma::desc_mnmajor(bb), b_lo = wgmma::desc_mnmajor(bb + B_BYTES);
         wgmma::fence();
 #pragma unroll
-        for (int k = 0; k < WG_KT / 16; ++k) {         // 16 pixels per k-step = 16 rows x 128 B = 2048 B = 128 descriptor units
-          const uint64_t o = (uint64_t)(k * 128);
+        for (int k = 0; k < WG_KT / 16; ++k) {         // 16 pixels per k-step
+          const uint64_t o = (uint64_t)k * wgmma::K16_STEP_MNMAJOR;
           wgmma::mma<BN, 1>(acc, a_hi + o, b_hi + o, (uint32_t)(!(first && k == 0)));
           wgmma::mma<BN, 1>(acc, a_lo + o, b_hi + o, 1u);
           wgmma::mma<BN, 1>(acc, a_hi + o, b_lo + o, 1u);
         }
       } else {                                          // plain bf16: one wgmma per k-step
-        const uint64_t a_d = wgmma::desc_sw128(base, WG_BOX, 1024u);
-        const uint64_t b_d = wgmma::desc_sw128(smem0 + (uint32_t)(s * STAGE) + (uint32_t)A_BYTES, WG_BOX, 1024u);
+        const uint64_t a_d = wgmma::desc_mnmajor(base);
+        const uint64_t b_d = wgmma::desc_mnmajor(smem0 + (uint32_t)(s * STAGE) + (uint32_t)A_BYTES);
         wgmma::fence();
 #pragma unroll
         for (int k = 0; k < WG_KT / 16; ++k) {
-          const uint64_t o = (uint64_t)(k * 128);
+          const uint64_t o = (uint64_t)k * wgmma::K16_STEP_MNMAJOR;
           wgmma::mma<BN, 1>(acc, a_d + o, b_d + o, (uint32_t)(!(first && k == 0)));
         }
       }

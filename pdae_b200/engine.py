@@ -302,6 +302,12 @@ class Plan:
             if fn == "gemm_tc2_softmax":
                 compiled.append(self._compile_gemm_softmax(args))
                 continue
+            if fn == "gemm_tc2_major":
+                compiled.append(self._compile_gemm_major(args))
+                continue
+            if fn == "gemm_tc2_softmax_grad":
+                compiled.append(self._compile_gemm_softmax_grad(args))
+                continue
             if fn == "conv_tc2_skip":
                 compiled.append(self._compile_tc2_skip(args))
                 continue
@@ -425,6 +431,25 @@ class Plan:
         self._tc2_handles.append(h)
         return (self.L.pdae_conv_tc2_run, [h, None], 1, "gemm_tc2")
 
+    def _compile_gemm_major(self, args):
+        a, a_mn, a_ld, a_bs, b, b_mn, b_ld, b_bs, out, o_ld, o_bs, batch, M, N, K = args
+        h = ctypes.c_void_p()
+        rc = self.L.pdae_gemm_tc2_create_major(ctypes.byref(h), self._resolve(a), a_mn, a_ld, a_bs, self._resolve(b), b_mn, b_ld,
+                                               b_bs, self._resolve(out), o_ld, o_bs, batch, M, N, K)
+        _native.check(rc, "pdae_gemm_tc2_create_major")
+        self._tc2_handles.append(h)
+        return (self.L.pdae_conv_tc2_run, [h, None], 1, "gemm_tc2_major")
+
+    def _compile_gemm_softmax_grad(self, args):
+        a, a_ld, a_bs, b, b_ld, b_bs, pr, p_ld, p_bs, out, o_ld, o_bs, batch, M, N, K, alpha = args
+        h = ctypes.c_void_p()
+        rc = self.L.pdae_gemm_tc2_softmax_grad_create(ctypes.byref(h), self._resolve(a), a_ld, a_bs, self._resolve(b), b_ld, b_bs,
+                                                      self._resolve(pr), p_ld, p_bs, self._resolve(out), o_ld, o_bs, batch, M, N,
+                                                      K, alpha)
+        _native.check(rc, "pdae_gemm_tc2_softmax_grad_create")
+        self._tc2_handles.append(h)
+        return (self.L.pdae_conv_tc2_run, [h, None], 1, "gemm_tc2_softmax_grad")
+
     def _compile_gemm(self, args):
         a, a_ld, a_bs, b, b_ld, b_bs, out, odt, o_ld, o_bs, batch, M, N, K = args
         h = ctypes.c_void_p()
@@ -435,9 +460,24 @@ class Plan:
         return (self.L.pdae_conv_tc2_run, [h, None], 1, "gemm_tc2")
 
     def gemm_tc(self, a, a_ld, a_bs, b, b_ld, b_bs, out, out_ld, out_bs, *, batch, M, N, K, out_dtype,
-                softmax_alpha: Optional[float] = None, flops: Optional[float] = None) -> None:
+                softmax_alpha: Optional[float] = None, flops: Optional[float] = None, a_mn: bool = False, b_mn: bool = False,
+                softmax_grad: Optional[tuple] = None) -> None:
         """Batched out_i = A_i (MxK) * B_i (NxK)^T on the persistent wgmma kernel; a/b/out are Buf or BufView.
-        softmax_alpha: store softmax_rows(alpha * out_i) (bf16) instead -- needs N in {64,128,256} (row inside one tile)."""
+        softmax_alpha: store softmax_rows(alpha * out_i) (bf16) instead -- needs N in {64,128,256} (row inside one tile).
+        a_mn / b_mn: that operand is stored MN-major, A_i as [K][M] / B_i as [K][N] with *_ld elements between k rows (fp32 out).
+        softmax_grad = (P, p_ld, p_bs, alpha): store alpha * P_i * (out_i - rowsum(P_i * out_i)) (bf16) instead, P_i being bf16
+        with the output's shape -- the attention backward's dS; K-major operands, N in {64,128,256}."""
+        if softmax_grad is not None:
+            pr, p_ld, p_bs, alpha = softmax_grad
+            assert out_dtype == torch.bfloat16 and N in (64, 128, 256) and softmax_alpha is None and not (a_mn or b_mn)
+            self.call("gemm_tc2_softmax_grad", a, a_ld, a_bs, b, b_ld, b_bs, pr, p_ld, p_bs, out, out_ld, out_bs, batch, M, N, K,
+                      ctypes.c_float(alpha), flops=2.0 * batch * M * N * K)
+            return
+        if a_mn or b_mn:
+            assert out_dtype == torch.float32 and softmax_alpha is None
+            self.call("gemm_tc2_major", a, int(a_mn), a_ld, a_bs, b, int(b_mn), b_ld, b_bs, out, out_ld, out_bs, batch, M, N, K,
+                      flops=2.0 * batch * M * N * K if flops is None else flops)
+            return
         if softmax_alpha is not None:
             assert out_dtype == torch.bfloat16 and N in (64, 128, 256)
             self.call("gemm_tc2_softmax", a, a_ld, a_bs, b, b_ld, b_bs, out, out_ld, out_bs, batch, M, N, K,
@@ -588,6 +628,16 @@ class Plan:
         with (e.g. the transposed, flipped weights of a dgrad) -- the packed copy still tracks the PARAMETER's version.
         Returns the per-channel (sum, sum^2) buffer [B][Cout][2] if the tensor-core epilogue produced one."""
         pad = k // 2 if pad is None else pad
+        if (self.train_tc == "bf16" and x.dtype == torch.bfloat16 and not (in_nchw or out_nchw or a_silu) and skip is None
+                and w_transform is None and pad == k // 2 and self._tc_shape_ok(Cin, Cout, k, stride, H, W)):
+            # an input that is already a plain bf16 tensor in a bf16 training forward (the attention block's normalised input and
+            # attention output): conv_tc2 reads it as it is, and it is its own copy for the backward's weight gradient
+            wp = self.pack((wkey or id(weight), "tc"), [weight],
+                           lambda: weight.detach().reshape(Cout, Cin, k * k).permute(2, 0, 1).to(torch.bfloat16))
+            x.tc_copy = x
+            self.call("conv_tc2", x, wp, self.param(bias), residual, out, _DT[out.dtype], None, B, H, W, Cin, Cout, k, 0,
+                      bn_override, flops=2.0 * B * H * W * Cout * Cin * k * k)
+            return None
         if (self.train_tc == "bf16" and stride == 2 and k == 3 and pad == 1 and x.dtype == torch.float32
                 and out.dtype == torch.float32 and not (in_nchw or out_nchw or a_silu) and skip is None and w_transform is None
                 and residual is None and self.L.pdae_conv_s2_tc_supported(H, W, Cin, Cout)):

@@ -464,17 +464,21 @@ class AttentionBlock(PlannedModule):
         ab = P.gn_coef(x.b1, C, None, 0, self.norm.weight, self.norm.bias, B=B, HW=T, stats1=x.s1)
         sums = P.last_sums
         tcq = P.use_tc(C, 3 * C, 1, 1, H, W)
-        xn, _ = P.gn_apply(x.b1, C, None, 0, ab, silu=False, resample=RESAMPLE_NONE, B=B, H=H, W=W,
-                           act_dtype=torch.bfloat16 if tcq else torch.float32)
         heads, ch = self.num_heads, C // self.num_heads
-        if tcq and P.can_gemm_tc(T, T, ch) and P.can_gemm_tc(T, ch, T):
+        # bf16 training forward (autocast): an eligible block runs the bf16 tensor-core attention below and keeps its bf16 qkv,
+        # probabilities and attention output for the tensor-core backward (train.Backward.attention)
+        amp = tape is not None and P.train_tc == "bf16" and self.amp_eligible(T, ch)
+        xn, _ = P.gn_apply(x.b1, C, None, 0, ab, silu=False, resample=RESAMPLE_NONE, B=B, H=H, W=W,
+                           act_dtype=torch.bfloat16 if (tcq or amp) else torch.float32)
+        if amp or (tcq and P.can_gemm_tc(T, T, ch) and P.can_gemm_tc(T, ch, T)):
             # ---- tensor-core attention: bf16 qkv -> S = Q K^T (batched wgmma GEMM) -> softmax -> P V ----
             qkv = P.new((B, T, 3 * C), torch.bfloat16, "qkv")
             P.conv(xn, self.qkv.weight, self.qkv.bias, qkv, B=B, H=H, W=W, Cin=C, Cout=3 * C, k=1)
             vT = P.new((B * heads, ch, T), torch.bfloat16, "vT")
             P.call("transpose_v", qkv, vT, B, T, C, heads, int(legacy), _STREAM)
             Pm = P.new((B * heads, T, T), torch.bfloat16, "att_probs")
-            att = P.new((B, T, C), torch.bfloat16, "att")
+            # (NHWC-shaped under amp: the backward's weight gradient of proj_out takes it as its bf16 input copy)
+            att = P.new((B, H, W, C) if amp else (B, T, C), torch.bfloat16, "att")
             hs_ = 3 * ch if legacy else ch                  # channel stride between heads inside a qkv row
             ko = ch if legacy else C                        # offset of K relative to Q
             alpha = 1.0 / math.sqrt(ch)                     # scale = ch^(-1/4) on both q and k (module.py:449-453)
@@ -493,6 +497,9 @@ class AttentionBlock(PlannedModule):
             for h in range(heads):
                 P.gemm_tc(Pm.at(h * T * T), T, heads * T * T, vT.at(h * ch * T), T, heads * ch * T,
                           att.at(h * ch), C, T * C, batch=B, M=T, N=ch, K=T, out_dtype=torch.bfloat16)
+            if amp:
+                tape.append(("attn", self, dict(x=x, ab=ab, sums=sums, xn=xn, qkv=qkv, probs=Pm, att=att, legacy=legacy,
+                                                tc=True)))
         elif tcq and tape is None and P.can_gemm_x3(T, T, ch) and P.can_gemm_x3(T, ch, T):
             # ---- split-operand tensor-core attention (fp32-grade): fp32 qkv -> [hi|lo|hi] x [hi|hi|lo] operand blocks ->
             # S = Q K^T (fp32) -> fp32 softmax, split -> A = P V (fp32); every product is three bf16 wgmma MMAs ----
@@ -531,6 +538,12 @@ class AttentionBlock(PlannedModule):
         os_ = P.conv(att, self.proj_out.weight, self.proj_out.bias, out, B=B, H=H, W=W, Cin=C, Cout=C, k=1, residual=x.b1,
                      want_stats=True)
         return Src(out, C, B, H, W, s1=os_)
+
+    @staticmethod
+    def amp_eligible(T: int, ch: int) -> bool:
+        """Does a block with T positions and ch channels per head train on the bf16 tensor-core attention under autocast?
+        T % 128 == 0 and T <= 256: a whole score row fits the softmax and softmax-gradient epilogues; ch % 64 == 0: whole k-blocks."""
+        return T % 128 == 0 and T <= 256 and ch % 64 == 0
 
     def forward(self, x):
         self._check_no_grad(x)

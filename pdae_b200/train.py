@@ -15,8 +15,11 @@ stride-2 / 3-channel convs stay fp32 on CUDA cores (``pdae_gn_bwd_*``, ``pdae_ge
 Mixed precision: a ShiftUNet / UNet training forward called inside ``torch.autocast("cuda")`` (the reference trainers'
 ``enable_amp``; either autocast dtype) builds separate bf16 trainers: the frozen half runs as a plain "bf16" plan, and the
 forward convs, data gradients and weight gradients of the trainable convs are single-pass bf16 MMAs with fp32 accumulation.
-Activations, GroupNorm, attention and every gradient stay fp32, so the reference's ``GradScaler`` works unchanged.  The
-semantic encoder does the same: under autocast its stride-2 convs (forward, data and weight gradient through parity views,
+An eligible attention block (T % 128 == 0, T <= 256, head width % 64 == 0) also runs its attention core on the tensor
+cores: bf16 qkv and probabilities in the forward; in the backward the softmax gradient sits in the epilogue of the dO V^T
+GEMM (``pdae_gemm_tc2_softmax_grad_create``) and dV / dQ / dK are GEMMs with MN-major operands
+(``pdae_gemm_tc2_create_major``) written in fp32 into the qkv gradient.  Other activations, GroupNorm and every gradient stay
+fp32, so the reference's ``GradScaler`` works unchanged.  The semantic encoder does the same: under autocast its stride-2 convs (forward, data and weight gradient through parity views,
 ``pdae_conv_tc2_create_s2*``, ``pdae_wgrad_tc_create_bf16_s2``) and its attention 1x1 convs are single-pass bf16 MMAs; its
 3-channel stem and final Linear stay fp32 on CUDA cores.  The latent MLP ignores autocast, and so does every forward-only
 call (sampling, ``infer_latents``, a frozen encoder).
@@ -285,14 +288,33 @@ class Backward:
         hs = 3 * ch if legacy else ch
         ko, vo = (ch, 2 * ch) if legacy else (C, 2 * C)
         d_qkv = P.new((B, T, 3 * C), torch.float32, "d_qkv")
+        alpha = 1.0 / math.sqrt(ch)
+        TT = T * T
+        if sv.get("tc") and P.precision == "bf16":
+            # bf16 tensor-core attention backward (the forward kept bf16 qkv and probabilities): dO in bf16 once, then per head
+            #   dS = alpha P (dO V^T - rowsum(P dO V^T))   (softmax gradient in the GEMM epilogue, bf16)
+            #   dV = P^T dO,  dQ = dS K,  dK = dS^T Q      (MN-major operands, fp32 straight into d_qkv)
+            d_o, _ = P.gn_apply(d_att, C, None, 0, None, silu=False, resample=RESAMPLE_NONE, B=B, H=H, W=W,
+                                act_dtype=torch.bfloat16)
+            dS = P.new((B * heads, T, T), torch.bfloat16, "att_dS")
+            for h in range(heads):
+                q, k, v, o = h * hs, h * hs + ko, h * hs + vo, h * ch
+                P.gemm_tc(d_o.at(o), C, T * C, qkv.at(v), row, T * row, dS.at(h * TT), T, heads * TT, batch=B, M=T, N=T, K=ch,
+                          out_dtype=torch.bfloat16, softmax_grad=(probs.at(h * TT), T, heads * TT, alpha))
+                P.gemm_tc(probs.at(h * TT), T, heads * TT, d_o.at(o), C, T * C, d_qkv.at(v), row, T * row, batch=B, M=T, N=ch,
+                          K=T, out_dtype=torch.float32, a_mn=True, b_mn=True)
+                P.gemm_tc(dS.at(h * TT), T, heads * TT, qkv.at(k), row, T * row, d_qkv.at(q), row, T * row, batch=B, M=T, N=ch,
+                          K=T, out_dtype=torch.float32, b_mn=True)
+                P.gemm_tc(dS.at(h * TT), T, heads * TT, qkv.at(q), row, T * row, d_qkv.at(k), row, T * row, batch=B, M=T, N=ch,
+                          K=T, out_dtype=torch.float32, a_mn=True, b_mn=True)
+            d_xn = self.conv(sv["xn"], d_qkv, blk.qkv.weight, blk.qkv.bias, B=B, H=H, W=W, Cin=C, Cout=3 * C, k=1)
+            return self.gn(x, sv["ab"], sv["sums"], blk.norm, d_xn, silu=False, resample=RESAMPLE_NONE, add=d_out, add_ld=C)
         dP = P.new((B * heads, T, T), torch.float32, "dP")
         i64 = ctypes.c_int64
-        alpha = 1.0 / math.sqrt(ch)
 
         def gemm(A, lda, abs_, ahs, tA, Bm, ldb, bbs, bhs, tB, Cc, ldc, cbs, chs, M, N, K, al=1.0):
             P.call("gemm_batched_simt", A, i64(lda), i64(abs_), i64(ahs), int(tA), Bm, i64(ldb), i64(bbs), i64(bhs), int(tB), Cc,
                    i64(ldc), i64(cbs), i64(chs), M, N, K, B, heads, F32(al), _STREAM)
-        TT = T * T
         # dV = P^T dO
         gemm(probs, T, heads * TT, TT, 1, d_att, C, T * C, ch, 0, d_qkv.at(vo), row, T * row, hs, T, ch, T)
         # dP = dO V^T
