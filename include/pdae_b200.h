@@ -137,6 +137,13 @@ int pdae_mlp_mod_ln_act(const float* h, const float* cond, const float* ln_w, co
                         int silu, float* out, int out_ld, int B, int N, pdae_stream_t stream);
 /* dst[b][col0 + j] = src[b][j], j < N (row strides dst_ld / N).                                       */
 int pdae_copy_cols(const float* src, float* dst, int dst_ld, int col0, int B, int N, pdae_stream_t stream);
+/* bf16 operands of the autocast latent training step.  pdae_mlp_mod_ln_act_bf16: cond row b at cond + b * cond_ld; with a
+ * mask the value is then multiplied by mask[b][j] * mask_scale; out (bf16) = bf16_rn of exactly what pdae_mlp_mod_ln_act
+ * followed by pdae_mul_mask_cols writes in fp32.  pdae_copy_cols_bf16: pdae_copy_cols into a bf16 dst.                  */
+int pdae_mlp_mod_ln_act_bf16(const float* h, const float* cond, int cond_ld, const float* ln_w, const float* ln_b, float eps,
+                             int silu, const float* mask, float mask_scale, void* out_bf16, int out_ld, int B, int N,
+                             pdae_stream_t stream);
+int pdae_copy_cols_bf16(const float* src, void* dst_bf16, int dst_ld, int col0, int B, int N, pdae_stream_t stream);
 
 
 /* ---- backward (training config: autograd through module.py:278-297,361-384,422-428 and the encoders), fp32 ---------
@@ -171,6 +178,14 @@ int pdae_mul_mask(float* a, const float* mask, float scale, int64_t n, pdae_stre
 int pdae_mlp_mod_ln_act_bwd(const float* h, const float* cond, const float* ln_w, const float* ln_b, float eps, int silu,
                             const float* dy, int dy_ld, float* dh, float* dcond, float* d_ln_w, float* d_ln_b, int B, int N,
                             pdae_stream_t stream);
+/* The same for the autocast step: cond and dcond rows at leading dimension cond_ld (a layer's column block of the bank),
+ * dy multiplied by mask[b][j] * mask_scale as it is read (mask may be NULL), and dh / dcond written in fp32 and, in the
+ * same pass, as their bf16 roundings (dh_bf16 [B][N], dcond_bf16 with leading dimension cond_ld).  The fp32 outputs equal
+ * pdae_mul_mask_cols + pdae_mlp_mod_ln_act_bwd's bit for bit.                                                        */
+int pdae_mlp_mod_ln_act_bwd_bf16(const float* h, const float* cond, int cond_ld, const float* ln_w, const float* ln_b, float eps,
+                                 int silu, const float* dy, int dy_ld, const float* mask, float mask_scale, float* dh,
+                                 void* dh_bf16, float* dcond, void* dcond_bf16, float* d_ln_w, float* d_ln_b, int B, int N,
+                                 pdae_stream_t stream);
 /* a[b][0..N) *= mask[b][0..N) * scale on a row-major [B][ld] matrix (dropout, mlp_skip_net.py:140, on the concat buffer). */
 int pdae_mul_mask_cols(float* a, int ld, const float* mask, float scale, int B, int N, pdae_stream_t stream);
 int pdae_nchw_to_nhwc(const float* src, float* dst, int B, int C, int HW, pdae_stream_t stream);
@@ -277,6 +292,11 @@ int pdae_conv_tc2_create_s2(pdae_conv_tc2_plan** plan, const void* in_bf16, cons
                             int B, int H, int W, int Cin, int Cout);
 int pdae_conv_tc2_create_s2_dgrad(pdae_conv_tc2_plan** plan, const void* dy_bf16, const void* wt_bf16, float* dx, int B, int H,
                                   int W, int Cin, int Cout);
+/* Split-K Linear (bf16 autocast latent training): out[B][Cout] (fp32) += in[B][Cin] (bf16) * w[Cout][Cin]^T (bf16) + bias.
+ * Each output tile's k range is split so that about one wave of (tile, k range) items covers the SMs; the partial tiles are
+ * added with fp32 reductions, so `out` must be zeroed before every run.  Cin, Cout multiples of 64.                     */
+int pdae_conv_tc2_create_splitk(pdae_conv_tc2_plan** plan, const void* in_bf16, const void* w_bf16, const float* bias, float* out,
+                                int B, int Cin, int Cout);
 int pdae_conv_tc2_run(const pdae_conv_tc2_plan* plan, pdae_stream_t stream);
 /* Image-head plans (cout_valid > 0): fuse the per-step DDIM update (diffusion/ddim.py:43-55,66-79,91-107,123-138) into the head's
  * epilogue.  fuse_desc_device: 8 x int64 in DEVICE memory, read at run time = { flags, eps*, x_t*, t*, tab_A*, tab_Bm*, tab_s1m*,

@@ -73,6 +73,8 @@ _SIGS = {
     "pdae_noise_p_sample": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int64, _P]),
     "pdae_mlp_mod_ln_act": (c_int, [_P, _P, _P, _P, c_float, c_int, _P, c_int, c_int, c_int, _P]),
     "pdae_copy_cols": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    "pdae_mlp_mod_ln_act_bf16": (c_int, [_P, _P, c_int, _P, _P, c_float, c_int, _P, c_float, _P, c_int, c_int, c_int, _P]),
+    "pdae_copy_cols_bf16": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     "pdae_conv2d_dgrad_simt": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_conv2d_wgrad_simt": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_colsum": (c_int, [_P, c_int64, c_int, _P, _P]),
@@ -105,6 +107,7 @@ _SIGS = {
     "pdae_conv_s2_tc_supported": (c_int, [c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_s2": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_s2_dgrad": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_conv_tc2_create_splitk": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, c_int, c_int]),
     "pdae_conv_tc2_run": (c_int, [_P, _P]),
     "pdae_conv_tc2_set_head_fuse": (c_int, [_P, _P]),
     "pdae_conv_tc3_supported": (c_int, [c_int, c_int, c_int, c_int]),
@@ -124,6 +127,8 @@ _SIGS = {
     "pdae_softmax_split3": (c_int, [_P, _P, c_int64, c_int, c_float, _P]),
     "pdae_conv_tc2_destroy": (None, [_P]),
     "pdae_mlp_mod_ln_act_bwd": (c_int, [_P, _P, _P, _P, c_float, c_int, _P, c_int, _P, _P, _P, _P, c_int, c_int, _P]),
+    "pdae_mlp_mod_ln_act_bwd_bf16": (c_int, [_P, _P, c_int, _P, _P, c_float, c_int, _P, c_int, _P, c_float, _P, _P, _P, _P, _P, _P,
+                                             c_int, c_int, _P]),
     "pdae_mul_mask_cols": (c_int, [_P, c_int, _P, c_float, c_int, c_int, _P]),
     "pdae_stem_conv_bf16": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_gn_apply_split3": (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P]),

@@ -449,17 +449,25 @@ __global__ void nchw_to_nhwc_kernel(const float* __restrict__ src, float* __rest
 // MLPLNAct backward (model/mlp_skip_net.py:123-141):  v = h*(1+c);  u = (v-mean)*rstd;  y0 = u*lw+lb;  y = SiLU(y0)
 // one CTA per row; mean / rstd recomputed like the forward kernel.  dy is read with leading dimension dy_ld (the
 // gradient of the skip-concat buffer's left columns).  dlw / dlb accumulate over rows with atomics (zero them first).
+// BF16 (the autocast training step): cond / dcond rows have leading dimension cond_ld (a column block of the layers' bank),
+// dy is multiplied by mask * scale as it is read (what pdae_mul_mask_cols does in place), and dh / dcond are also stored as
+// bf16 (the GEMM operands of the data and weight gradients) next to their fp32 values.
+template <bool BF16>
 __global__ void __launch_bounds__(256) mlp_mod_ln_act_bwd_kernel(const float* __restrict__ h, const float* __restrict__ cond,
-                                                                 const float* __restrict__ lw, const float* __restrict__ lb,
-                                                                 float eps, int silu, const float* __restrict__ dy, int dy_ld,
-                                                                 float* __restrict__ dh, float* __restrict__ dcond,
+                                                                 int cond_ld, const float* __restrict__ lw,
+                                                                 const float* __restrict__ lb, float eps, int silu,
+                                                                 const float* __restrict__ dy, int dy_ld,
+                                                                 const float* __restrict__ mask, float scale,
+                                                                 float* __restrict__ dh, __nv_bfloat16* __restrict__ dh_bf,
+                                                                 float* __restrict__ dcond, __nv_bfloat16* __restrict__ dcond_bf,
                                                                  float* __restrict__ dlw, float* __restrict__ dlb, int N) {
   __shared__ float red[2][8];
   __shared__ float bc[2];
   const int b = blockIdx.x;
   const float* hr = h + (long long)b * N;
-  const float* cr = cond ? cond + (long long)b * N : nullptr;
+  const float* cr = cond ? cond + (long long)b * cond_ld : nullptr;
   const float* gr = dy + (long long)b * dy_ld;
+  const float* mr = BF16 && mask ? mask + (long long)b * N : nullptr;
   auto block_sum2 = [&](float a, float c2, float& oa, float& oc) {
 #pragma unroll
     for (int o = 16; o > 0; o >>= 1) {
@@ -512,6 +520,7 @@ __global__ void __launch_bounds__(256) mlp_mod_ln_act_bwd_kernel(const float* __
     const float u = lw ? (v - mean) * rstd : v;
     const float y0 = lw ? u * lw[j] + lb[j] : u;
     float g = gr[j];
+    if (mr) g *= mr[j] * scale;
     if (silu) {
       const float sg = 1.0f / (1.0f + expf(-y0));
       g *= sg * (1.0f + y0 * (1.0f - sg));
@@ -536,14 +545,21 @@ __global__ void __launch_bounds__(256) mlp_mod_ln_act_bwd_kernel(const float* __
     const float u = lw ? (v - mean) * rstd : v;
     const float y0 = lw ? u * lw[j] + lb[j] : u;
     float g = gr[j];
+    if (mr) g *= mr[j] * scale;
     if (silu) {
       const float sg = 1.0f / (1.0f + expf(-y0));
       g *= sg * (1.0f + y0 * (1.0f - sg));
     }
     float dv = g;
     if (lw) dv = rstd * (g * lw[j] - m1 - u * m2);
-    dh[(long long)b * N + j] = dv * (1.0f + cv);
-    if (dcond) dcond[(long long)b * N + j] = dv * hv;
+    const float dhv = dv * (1.0f + cv);
+    dh[(long long)b * N + j] = dhv;
+    if (BF16) dh_bf[(long long)b * N + j] = __float2bfloat16_rn(dhv);
+    if (dcond) {
+      const float dcv = dv * hv;
+      dcond[(long long)b * cond_ld + j] = dcv;
+      if (BF16) dcond_bf[(long long)b * cond_ld + j] = __float2bfloat16_rn(dcv);
+    }
   }
 }
 
@@ -792,9 +808,24 @@ extern "C" int pdae_mlp_mod_ln_act_bwd(const float* h, const float* cond, const 
   PDAE_REQUIRE(h && dy && dh && B > 0 && N > 0 && dy_ld >= N, "mlp_mod_ln_act_bwd: bad args");
   PDAE_REQUIRE(!ln_w || ln_b, "mlp_mod_ln_act_bwd: LayerNorm weight without bias");
   PDAE_REQUIRE(!dcond || cond, "mlp_mod_ln_act_bwd: dcond without cond");
-  mlp_mod_ln_act_bwd_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, ln_w, ln_b, eps, silu, dy, dy_ld, dh, dcond, d_ln_w,
-                                                                 d_ln_b, N);
+  mlp_mod_ln_act_bwd_kernel<false><<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, N, ln_w, ln_b, eps, silu, dy, dy_ld, nullptr,
+                                                                        1.0f, dh, nullptr, dcond, nullptr, d_ln_w, d_ln_b, N);
   PDAE_LAUNCH_CHECK("mlp_mod_ln_act_bwd_kernel");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_mlp_mod_ln_act_bwd_bf16(const float* h, const float* cond, int cond_ld, const float* ln_w, const float* ln_b,
+                                            float eps, int silu, const float* dy, int dy_ld, const float* mask, float mask_scale,
+                                            float* dh, void* dh_bf16, float* dcond, void* dcond_bf16, float* d_ln_w, float* d_ln_b,
+                                            int B, int N, pdae_stream_t stream) {
+  PDAE_REQUIRE(h && dy && dh && dh_bf16 && B > 0 && N > 0 && dy_ld >= N, "mlp_mod_ln_act_bwd_bf16: bad args");
+  PDAE_REQUIRE(!ln_w || ln_b, "mlp_mod_ln_act_bwd_bf16: LayerNorm weight without bias");
+  PDAE_REQUIRE(!dcond || (cond && dcond_bf16), "mlp_mod_ln_act_bwd_bf16: dcond without cond or its bf16 copy");
+  PDAE_REQUIRE(!cond || cond_ld >= N, "mlp_mod_ln_act_bwd_bf16: cond_ld=%d < N=%d", cond_ld, N);
+  mlp_mod_ln_act_bwd_kernel<true><<<B, 256, 0, (cudaStream_t)stream>>>(
+      h, cond, cond_ld, ln_w, ln_b, eps, silu, dy, dy_ld, mask, mask_scale, dh, (__nv_bfloat16*)dh_bf16, dcond,
+      (__nv_bfloat16*)dcond_bf16, d_ln_w, d_ln_b, N);
+  PDAE_LAUNCH_CHECK("mlp_mod_ln_act_bwd_kernel<bf16>");
   return PDAE_OK;
 }
 

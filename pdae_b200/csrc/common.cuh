@@ -82,5 +82,7 @@ template <>
 __device__ __forceinline__ float load1<__nv_bfloat16>(const __nv_bfloat16* p) {
   return __bfloat162float(*p);
 }
+__device__ __forceinline__ void store1(float* p, float v) { *p = v; }
+__device__ __forceinline__ void store1(__nv_bfloat16* p, float v) { *p = __float2bfloat16_rn(v); }
 
 }  // namespace pdae

@@ -30,6 +30,11 @@
 // with P (bf16, the forward's probabilities) read for the same rows and columns, so dP never leaves the registers.  A 256-wide
 // row does not fit one warpgroup's registers beside the epilogue: with GM_SPLITN the tile is 64 rows x 2 BN columns, both
 // warpgroups reading the same A rows, warpgroup g computing columns [g BN, g BN + BN); the row sums meet in shared memory.
+//
+// GM_SPLITK: split-K for the Linear shape (H = W = 1, 1x1, M = batch), whose few output tiles would leave most SMs idle.  A
+// work item is (tile, k range): item = tile * splitk + split covers k-blocks [split kchunk, split kchunk + kchunk).  Each
+// item adds its partial tile into the zeroed fp32 output with red.global.add straight from the accumulator fragments
+// (rows past the batch skipped), split 0 adding the bias as well.  fp32 output only: no residual, statistics or bf16 store.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -44,12 +49,12 @@ constexpr int T2_STG_BYTES = 128 * 128;        // staging tile: 128 rows x 128 B
 constexpr int T2_MAX_STAGES = 8;
 constexpr int T2_THREADS = 288;   // warps 0-7: two consumer warpgroups, warp 8: TMA producer
 constexpr int T2_CONSUMERS = 256;
-constexpr int GM_A_MN = 1, GM_B_MN = 2, GM_SMGRAD = 4, GM_SPLITN = 8;   // conv_tc2_kernel's GM bits (kernel header)
+constexpr int GM_A_MN = 1, GM_B_MN = 2, GM_SMGRAD = 4, GM_SPLITN = 8, GM_SPLITK = 16;   // conv_tc2_kernel's GM bits (kernel header)
 
 struct ConvTc2Args {
   const float* bias;
   float* ch_stats;    // [B][Cout][2] fp32 partial (sum, sum^2) accumulators or nullptr
-  float* out_nchw;    // BN==16 head: NCHW fp32 output
+  float* out_nchw;    // BN==16 head: NCHW fp32 output; GM_SPLITK: the zeroed [B][Cout] fp32 output the partial tiles are added to
   const long long* fuse;  // BN==16 head: optional device-side descriptor of the fused DDIM update (see pdae_conv_tc2_set_head_fuse)
   int B, H, W, Cout;
   int tw, th, tn;
@@ -64,6 +69,7 @@ struct ConvTc2Args {
                   // region and reused by all of the CTA's tiles; pipeline stages then hold A tiles only
   float softmax_alpha;  // > 0: the epilogue stores softmax_row(alpha * acc) (bf16) instead of acc -- attention scores whose
                         // whole row lives in this tile's accumulators (N == BN); model/module.py:452-455,483-486
+  int splitk, kchunk;   // GM_SPLITK: k ranges per tile, k-blocks per range
 };
 // GM_SMGRAD operands (a kernel parameter of its own: ConvTc2Args keeps its size, so the other modes compile as before)
 struct SmGradArgs {
@@ -173,6 +179,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   __shared__ float st_part[2][8][32];              // per-chunk partial sums [sum | sum^2][row run][column] (CW * 8 runs / 32)
 
   constexpr bool SPN = (GM & GM_SPLITN) != 0;   // 64-row tiles, the B tile holds 2 BN rows (one BN-row half per warpgroup)
+  constexpr bool SK = (GM & GM_SPLITK) != 0;    // work item = (tile, k range); partial tiles reduced into the output
   constexpr int B_BYTES = (SPN ? 2 : 1) * BN * T2_BK * 2;
   constexpr int STAGE_BYTES = T2_A_BYTES + ((B_BYTES + 1023) / 1024) * 1024;
   constexpr int CW = OB ? 64 : 32;             // accumulator columns per staging tile (128-byte rows)
@@ -230,7 +237,8 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     }
     for (int tile = tile_begin; tile < tile_end; ++tile) {
       const int ph2 = S2 == 2 ? (tile & 3) : 0;      // stride-2 dgrad: sub-pixel phase of this tile
-      const int tl = S2 == 2 ? (tile >> 2) : tile;
+      const int tl = S2 == 2 ? (tile >> 2) : (SK ? tile / p.splitk : tile);
+      const int kb0 = SK ? (tile - tl * p.splitk) * p.kchunk : 0;   // split-K: first k-block of this item
       const int nt = tl / p.tiles_m;
       int mt = tl - nt * p.tiles_m;
       const int tx = mt % p.tiles_x;
@@ -267,8 +275,9 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
         }
         continue;
       }
-      int tap = 0, kb = 0, dy = p.ksize == 3 ? -1 : 0, dx = dy;
-      for (int it = 0; it < total_k; ++it) {
+      int tap = 0, kb = kb0, dy = p.ksize == 3 ? -1 : 0, dx = dy;
+      const int n_main = SK ? min(p.kchunk, p.kblocks - kb0) : total_k;
+      for (int it = 0; it < n_main; ++it) {
         mb_wait(s_u32(&bar_empty[s]), ph ^ 1u);
         const uint32_t full = s_u32(&bar_full[s]);
         const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
@@ -331,7 +340,8 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
     if (p.w_stat && tile_begin < tile_end) mb_wait(s_u32(&bar_w), 0u);   // stationary weights have landed
     for (int tile = tile_begin; tile < tile_end; ++tile) {
       const int ph2 = S2 == 2 ? (tile & 3) : 0;
-      const int tl = S2 == 2 ? (tile >> 2) : tile;
+      const int tl = S2 == 2 ? (tile >> 2) : (SK ? tile / p.splitk : tile);
+      const int kb0 = SK ? (tile - tl * p.splitk) * p.kchunk : 0;
       const int nt = tl / p.tiles_m;
       int mt = tl - nt * p.tiles_m;
       const int tx = mt % p.tiles_x;
@@ -339,7 +349,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       const int ty = mt % p.tiles_y;
       const int bt = mt / p.tiles_y;
       const int x0 = tx * p.tw, y0 = ty * p.th, b0 = bt * p.tn, n0 = nt * BN;
-      const int n_it = S2 == 2 ? s2_phase_taps(ph2) * p.kblocks : total_all;
+      const int n_it = S2 == 2 ? s2_phase_taps(ph2) * p.kblocks : (SK ? min(p.kchunk, p.kblocks - kb0) : total_all);
       if constexpr (BN != 16) {
         if (p.has_res && elected) {            // residual chunk 0 of this tile (lands while the main loop runs)
           mb_expect_tx(rbar, T2_STG_BYTES);
@@ -351,7 +361,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       for (int it = 0; it < n_it; ++it) {
         mb_wait(s_u32(&bar_full[s]), ph);
         const uint32_t sa = smem0 + (uint32_t)s * stage_stride;
-        if constexpr (GM == 0) {
+        if constexpr ((GM & ~GM_SPLITK) == 0) {
           const uint64_t ad = wgmma::desc_sw128(sa + (uint32_t)wg * (64u * 128u), 16u, 1024u);
           const uint64_t bd = wgmma::desc_sw128(p.w_stat ? wbase + (uint32_t)(it * B_BYTES) : sa + T2_A_BYTES, 16u, 1024u);
           wgmma::fence();
@@ -380,6 +390,23 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       wgmma::wait<0>();
       if (prev >= 0 && lane == 0) mb_arrive(s_u32(&bar_empty[prev]));
 
+      if constexpr (SK) {
+        // split-K partial tile (H = W = 1: tile row r is batch row b0 + r): fp32 reductions into the zeroed output
+        const bool add_bias = p.bias != nullptr && kb0 == 0;
+#pragma unroll
+        for (int i = 0; i < BN / 2; i += 2) {
+          const int b = b0 + 64 * wg + wgmma::frag_row(t, i), col = n0 + wgmma::frag_col(t, i);
+          float v0 = acc[i], v1 = acc[i + 1];
+          if (add_bias) {
+            const float2 bv = __ldg(reinterpret_cast<const float2*>(p.bias + col));
+            v0 += bv.x; v1 += bv.y;
+          }
+          if (b < p.B)
+            asm volatile("red.global.add.v2.f32 [%0], {%1, %2};" ::"l"(p.out_nchw + (long long)b * p.Cout + col), "f"(v0), "f"(v1)
+                         : "memory");
+        }
+        continue;
+      }
       if constexpr (BN == 16) {
         // ---- image head: first cout_valid columns -> NCHW fp32 planes ----
         const long long hw = (long long)p.H * p.W;
@@ -748,6 +775,10 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
   PDAE_REQUIRE(head ? (Cout == 16 && cout_valid <= 16 && d.out_dtype == PDAE_F32 && !d.residual && !d.ch_stats) : (Cout % 64 == 0),
                "conv_tc2_create: unsupported Cout=%d (cout_valid=%d)", Cout, cout_valid);
   PDAE_REQUIRE(d.out_dtype == PDAE_F32 || d.out_dtype == PDAE_BF16, "conv_tc2_create: bad out dtype");
+  PDAE_REQUIRE(!(d.gm & GM_SPLITK) || (H == 1 && W == 1 && ksize == 1 && !head && d.out_dtype == PDAE_F32 && !d.residual &&
+                                       !d.ch_stats && !d.Cin2 && !d.w_batched && d.s2 == 0 && d.softmax_alpha == 0.f),
+               "conv_tc2_create: split-K takes the Linear shape (H = W = 1, 1x1) with an fp32 output and no residual, "
+               "statistics or fused skip");
   // (a residual is read in the output's dtype: fp32 with an fp32 output, bf16 with a bf16 output)
   PDAE_REQUIRE(((uintptr_t)d.in & 15) == 0 && ((uintptr_t)d.w & 15) == 0 && ((uintptr_t)d.out & 15) == 0 &&
                    ((uintptr_t)d.residual & 15) == 0 && ((uintptr_t)d.bias & 15) == 0,
@@ -804,6 +835,14 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
   pl->gm = d.gm;
   pl->sg.p = static_cast<const __nv_bfloat16*>(d.sg_p); pl->sg.ld = d.sg_ld; pl->sg.bs = d.sg_bs; pl->sg.alpha = d.sg_alpha;
   a.tiles_total = a.tiles_m * (head ? 1 : Cout / (spn ? 2 * BN : BN)) * (d.s2 == 2 ? 4 : 1);   // stride-2 dgrad: x 4 phases
+  if (d.gm & GM_SPLITK) {
+    // about one wave of (tile, k range) items; every range non-empty
+    const int want = a.tiles_total >= g_num_sms ? 1 : g_num_sms / a.tiles_total;
+    a.kchunk = (a.kblocks + want - 1) / want;
+    a.splitk = (a.kblocks + a.kchunk - 1) / a.kchunk;
+    a.tiles_total *= a.splitk;
+    a.out_nchw = static_cast<float*>(d.out);
+  }
   const int b_bytes = ((BN * T2_BK * 2 + 1023) / 1024) * 1024 * (spn ? 2 : 1);
   int stage_bytes = T2_A_BYTES + b_bytes;
   const int staging = head ? 0 : (a.has_res ? 2 : 1) * T2_STG_BYTES;
@@ -815,7 +854,8 @@ static int tc2_create(pdae_conv_tc2_plan** plan_out, const Tc2Desc& d) {
   int wbytes = 0;
   a.w_stat = 0;
   // (not for the stride-2 dgrad: its phases read different subsets of the taps)
-  if (!head && !d.w_batched && d.s2 != 2 && Cout == BN && b_bytes == BN * T2_BK * 2 && a.tiles_total >= 2 * pl->grid) {
+  if (!head && !d.w_batched && d.s2 != 2 && !(d.gm & GM_SPLITK) && Cout == BN && b_bytes == BN * T2_BK * 2 &&
+      a.tiles_total >= 2 * pl->grid) {
     const int wb = total_all * b_bytes;
     if ((220 * 1024 - 1024 - staging - wb) / T2_A_BYTES >= 4) {
       a.w_stat = 1;
@@ -1087,6 +1127,22 @@ extern "C" int pdae_gemm_tc2_softmax_grad_create(pdae_conv_tc2_plan** plan_out, 
   return tc2_create(plan_out, d);
 }
 
+// Split-K Linear: out[B][Cout] (fp32) += in[B][Cin] (bf16) * w[Cout][Cin]^T (bf16) (+ bias), the k ranges of each output tile
+// spread over the SMs (kernel header).  `out` must be zeroed before every run.
+extern "C" int pdae_conv_tc2_create_splitk(pdae_conv_tc2_plan** plan_out, const void* in_bf16, const void* w_bf16,
+                                           const float* bias, float* out, int B, int Cin, int Cout) {
+  PDAE_REQUIRE(B > 0 && Cin > 0 && Cout > 0 && Cout % 64 == 0, "conv_tc2_create_splitk: B=%d Cin=%d Cout=%d: need Cout %% 64 == 0",
+               B, Cin, Cout);
+  Tc2Desc d;
+  d.in = in_bf16; d.w = w_bf16; d.bias = bias; d.residual = nullptr; d.out = out; d.out_dtype = PDAE_F32;
+  d.ch_stats = nullptr; d.B = B; d.H = 1; d.W = 1; d.Cin = Cin; d.Cout = Cout; d.ksize = 1; d.cout_valid = 0; d.bn_override = 0;
+  d.in_ld = Cin; d.in_bs = Cin;
+  d.w_batched = 0; d.w_ld = Cin; d.w_bs = (long long)Cout * Cin;
+  d.out_ld = Cout; d.out_bs = Cout;
+  d.gm = GM_SPLITK;
+  return tc2_create(plan_out, d);
+}
+
 // ---- 3x3, stride-2, pad-1 convs on plain bf16 operands (the semantic encoder's bf16 autocast training step) ----------------
 // H, W: the conv's INPUT size (even); the output / dY grid is H/2 x W/2.  Every tile shape the 128- and 64-pixel boxes of
 // conv_tc2 / wgrad_tc need exists for such a grid (power-of-two tiles, several images per box when the grid is small).
@@ -1150,7 +1206,8 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
 #define T2_GO_GM(BN, OB, GM) \
   launch_tc2<BN, OB, 0, GM>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
   const bool ob = pl->args.out_bf16 != 0;
-  if (pl->gm == (GM_SMGRAD | GM_SPLITN)) e = T2_GO_GM(128, true, GM_SMGRAD | GM_SPLITN);
+  if (pl->gm == GM_SPLITK) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_SPLITK) : T2_GO_GM(64, false, GM_SPLITK);
+  else if (pl->gm == (GM_SMGRAD | GM_SPLITN)) e = T2_GO_GM(128, true, GM_SMGRAD | GM_SPLITN);
   else if (pl->gm == GM_SMGRAD) e = pl->BN == 128 ? T2_GO_GM(128, true, GM_SMGRAD) : T2_GO_GM(64, true, GM_SMGRAD);
   else if (pl->gm == GM_A_MN) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_A_MN) : T2_GO_GM(64, false, GM_A_MN);
   else if (pl->gm == GM_B_MN) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_B_MN) : T2_GO_GM(64, false, GM_B_MN);

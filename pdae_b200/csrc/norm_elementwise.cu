@@ -541,15 +541,19 @@ __global__ void noise_p_sample_kernel(const float* __restrict__ x, const float* 
   }
 }
 
-// one CTA per row: y = act(LN(h*(1+cond)))
+// one CTA per row: y = act(LN(h*(1+cond))) (* mask * scale, the inverted dropout of pdae_mul_mask_cols); cond row b at
+// cond + b * cond_ld.  OutT = float: pdae_mlp_mod_ln_act.  OutT = bf16: the next Linear's tensor-core operand, bf16_rn of
+// exactly the fp32 value (same reduction order, same expressions).
+template <typename OutT>
 __global__ void __launch_bounds__(256) mlp_mod_ln_act_kernel(const float* __restrict__ h, const float* __restrict__ cond,
-                                                             const float* __restrict__ lw, const float* __restrict__ lb,
-                                                             float eps, int silu, float* __restrict__ out, int out_ld,
-                                                             int N) {
+                                                             int cond_ld, const float* __restrict__ lw,
+                                                             const float* __restrict__ lb, float eps, int silu,
+                                                             const float* __restrict__ mask, float scale,
+                                                             OutT* __restrict__ out, int out_ld, int N) {
   __shared__ float red[2][8];
   const int b = blockIdx.x;
   const float* hr = h + (long long)b * N;
-  const float* cr = cond ? cond + (long long)b * N : nullptr;
+  const float* cr = cond ? cond + (long long)b * cond_ld : nullptr;
   float s = 0.f, q = 0.f;
   for (int j = threadIdx.x; j < N; j += 256) {
     float v = hr[j];
@@ -579,16 +583,18 @@ __global__ void __launch_bounds__(256) mlp_mod_ln_act_kernel(const float* __rest
     if (cr) v = v * (1.0f + cr[j]);
     if (lw) v = (v - mean) * rstd * lw[j] + lb[j];
     if (silu) v = silu_f(v);
-    out[(long long)b * out_ld + j] = v;
+    if (mask) v *= mask[(long long)b * N + j] * scale;
+    store1(out + (long long)b * out_ld + j, v);
   }
 }
 
-__global__ void copy_cols_kernel(const float* __restrict__ src, float* __restrict__ dst, int dst_ld, int col0, int B,
+template <typename OutT>
+__global__ void copy_cols_kernel(const float* __restrict__ src, OutT* __restrict__ dst, int dst_ld, int col0, int B,
                                  int N) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)B * N) return;
   const int b = (int)(i / N), j = (int)(i % N);
-  dst[(long long)b * dst_ld + col0 + j] = src[i];
+  store1(dst + (long long)b * dst_ld + col0 + j, src[i]);
 }
 
 }  // namespace pdae
@@ -848,14 +854,34 @@ extern "C" int pdae_mlp_mod_ln_act(const float* h, const float* cond, const floa
                                    int silu, float* out, int out_ld, int B, int N, pdae_stream_t stream) {
   PDAE_REQUIRE(h && out && B > 0 && N > 0 && out_ld >= N, "mlp_mod_ln_act: bad args");
   PDAE_REQUIRE(!ln_w || ln_b, "mlp_mod_ln_act: LayerNorm weight without bias");
-  mlp_mod_ln_act_kernel<<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, ln_w, ln_b, eps, silu, out, out_ld, N);
+  mlp_mod_ln_act_kernel<float><<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, N, ln_w, ln_b, eps, silu, nullptr, 1.0f, out,
+                                                                    out_ld, N);
   PDAE_LAUNCH_CHECK("mlp_mod_ln_act_kernel");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_mlp_mod_ln_act_bf16(const float* h, const float* cond, int cond_ld, const float* ln_w, const float* ln_b,
+                                        float eps, int silu, const float* mask, float mask_scale, void* out_bf16, int out_ld,
+                                        int B, int N, pdae_stream_t stream) {
+  PDAE_REQUIRE(h && out_bf16 && B > 0 && N > 0 && out_ld >= N && (!cond || cond_ld >= N), "mlp_mod_ln_act_bf16: bad args");
+  PDAE_REQUIRE(!ln_w || ln_b, "mlp_mod_ln_act_bf16: LayerNorm weight without bias");
+  mlp_mod_ln_act_kernel<__nv_bfloat16><<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, cond_ld, ln_w, ln_b, eps, silu, mask,
+                                                                            mask_scale, (__nv_bfloat16*)out_bf16, out_ld, N);
+  PDAE_LAUNCH_CHECK("mlp_mod_ln_act_kernel<bf16>");
   return PDAE_OK;
 }
 
 extern "C" int pdae_copy_cols(const float* src, float* dst, int dst_ld, int col0, int B, int N, pdae_stream_t stream) {
   PDAE_REQUIRE(src && dst && col0 >= 0 && col0 + N <= dst_ld, "copy_cols: bad args");
-  copy_cols_kernel<<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(src, dst, dst_ld, col0, B, N);
+  copy_cols_kernel<float><<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(src, dst, dst_ld, col0, B, N);
   PDAE_LAUNCH_CHECK("copy_cols_kernel");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_copy_cols_bf16(const float* src, void* dst_bf16, int dst_ld, int col0, int B, int N, pdae_stream_t stream) {
+  PDAE_REQUIRE(src && dst_bf16 && B > 0 && N > 0 && col0 >= 0 && col0 + N <= dst_ld, "copy_cols_bf16: bad args");
+  copy_cols_kernel<__nv_bfloat16><<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(
+      src, (__nv_bfloat16*)dst_bf16, dst_ld, col0, B, N);
+  PDAE_LAUNCH_CHECK("copy_cols_kernel<bf16>");
   return PDAE_OK;
 }

@@ -81,6 +81,9 @@ class BufView:
     def __init__(self, buf: Buf, off: int):
         self.buf, self.off = buf, int(off)
 
+    def at(self, elem_offset: int) -> "BufView":
+        return BufView(self.buf, self.off + elem_offset)
+
 
 class Packed:
     """A derived (re-laid-out / converted) copy of parameters, refreshed when a source changes."""
@@ -320,6 +323,9 @@ class Plan:
             if fn in ("conv_tc2_s2", "conv_tc2_s2_dgrad", "wgrad_tc_bf16_s2"):
                 compiled.append(self._compile_s2(fn, args))
                 continue
+            if fn == "conv_tc2_splitk":
+                compiled.append(self._compile_splitk(args))
+                continue
             cargs = []
             sidx = -1
             for k, a in enumerate(args):
@@ -421,6 +427,15 @@ class Plan:
             return (self.L.pdae_wgrad_tc_run, [h, None], 1, fn)
         self._tc2_handles.append(h)
         return (self.L.pdae_conv_tc2_run, [h, None], 1, fn)
+
+    def _compile_splitk(self, args):
+        x, w, bias, out, B, Cin, Cout = args
+        h = ctypes.c_void_p()
+        rc = self.L.pdae_conv_tc2_create_splitk(ctypes.byref(h), self._resolve(x), self._resolve(w), self._resolve(bias),
+                                                self._resolve(out), B, Cin, Cout)
+        _native.check(rc, "pdae_conv_tc2_create_splitk")
+        self._tc2_handles.append(h)
+        return (self.L.pdae_conv_tc2_run, [h, None], 1, "conv_tc2_splitk")
 
     def _compile_gemm_softmax(self, args):
         a, a_ld, a_bs, b, b_ld, b_bs, out, o_ld, o_bs, batch, M, N, K, alpha = args
@@ -792,6 +807,22 @@ class Plan:
         """Linear with an already packed fp32 [Cin][Cout] weight (e.g. all blocks' emb layers concatenated)."""
         self.call("conv2d_simt", x, PDAE_F32, 0, wp, bias, None, out, 0, B, 1, 1, Cin, Cout, 1, 1, 0, int(a_silu), _STREAM,
                   flops=2.0 * B * Cin * Cout)
+
+    def linear_tc(self, x, wp: Buf, bias: Optional[Buf], *, B, Cin, Cout, name="linear_tc"):
+        """out[B][Cout] (fp32) = x[B][Cin] (bf16) wp[Cout][Cin]^T (bf16) + bias, one bf16 MMA per product on conv_tc2; returns
+        out.  When the output tiles alone would leave SMs idle (the latent MLP's Linears at training batch sizes: one 128-row
+        tile row) it runs split-K (pdae_conv_tc2_create_splitk): out is then a slice of the plan's zeroed arena, which the
+        plan's leading pdae_zero op clears on every replay, and the partial tiles are added into it."""
+        assert Cin % 64 == 0 and Cout % 64 == 0, (Cin, Cout)
+        fl = 2.0 * B * Cin * Cout
+        tiles = -(-B // 128) * (Cout // (128 if Cout % 128 == 0 else 64))   # = conv_tc2's output tiles
+        if tiles < torch.cuda.get_device_properties(self.device).multi_processor_count:
+            out = self.new_zeroed(B * Cout)
+            self.call("conv_tc2_splitk", x, wp, bias, out, B, Cin, Cout, flops=fl)
+            return out
+        out = self.new((B, Cout), torch.float32, name)
+        self.call("conv_tc2", x, wp, bias, None, out, PDAE_F32, None, B, 1, 1, Cin, Cout, 1, 0, 0, flops=fl)
+        return out
 
     def head_conv(self, x: Buf, weight: torch.Tensor, bias: torch.Tensor, out_nchw: Buf, *, B, H, W, Cin, Cout,
                   fuse_key: Optional[str] = None) -> None:

@@ -21,8 +21,11 @@ GEMM (``pdae_gemm_tc2_softmax_grad_create``) and dV / dQ / dK are GEMMs with MN-
 (``pdae_gemm_tc2_create_major``) written in fp32 into the qkv gradient.  Other activations, GroupNorm and every gradient stay
 fp32, so the reference's ``GradScaler`` works unchanged.  The semantic encoder does the same: under autocast its stride-2 convs (forward, data and weight gradient through parity views,
 ``pdae_conv_tc2_create_s2*``, ``pdae_wgrad_tc_create_bf16_s2``) and its attention 1x1 convs are single-pass bf16 MMAs; its
-3-channel stem and final Linear stay fp32 on CUDA cores.  The latent MLP ignores autocast, and so does every forward-only
-call (sampling, ``infer_latents``, a frozen encoder).
+3-channel stem and final Linear stay fp32 on CUDA cores.  The latent MLPSkipNet's training step under autocast runs every
+Linear but time_embed as a bf16 MMA (split-K where the batch leaves SMs idle), its layers' linear_emb as one bank GEMM, and
+writes each layer's bf16 GEMM operand from the fused modulate / LayerNorm / SiLU / dropout kernel (MLPTrainer._init_amp);
+an MLPSkipNet whose widths are not multiples of 64 keeps the fp32 trainer.  Every forward-only call (sampling,
+``infer_latents``, a frozen encoder, MLPSkipNet sampling) ignores autocast.
 """
 from __future__ import annotations
 
@@ -814,12 +817,31 @@ def encoder_train_forward(enc, x):
 # ======================================================================================================================
 # MLPSkipNet (latent DPM training, diffusion/gaussian_diffusion.py:373-398)
 # ======================================================================================================================
+def mlp_amp_supported(net) -> bool:
+    """Every Linear of the MLPSkipNet except time_embed has Cin and Cout in {D, Wd, Wd + D}: multiples of 64 put them all on
+    the tensor cores, which the bf16 trainer needs."""
+    return net.input_channel % 64 == 0 and net.model_channel % 64 == 0 and len(net.layers) >= 2
+
+
+def _tensor_of(b, shape) -> torch.Tensor:
+    """The tensor behind a plan buffer or a view of one (a split-K output lives in the plan's zeroed arena)."""
+    if isinstance(b, BufView):
+        return b.buf.tensor[b.off: b.off + int(np.prod(shape))].view(shape)
+    return b.tensor
+
+
 class MLPTrainer(_Generation):
     """Forward plan keeping every layer's (input, pre-activation, modulation) + backward plan for all parameters of the
-    MLPSkipNet; no gradient w.r.t. z_t (the reference's z_t is built from detached latents)."""
+    MLPSkipNet; no gradient w.r.t. z_t (the reference's z_t is built from detached latents).  `amp`: the bf16 plans of a
+    forward under autocast (_init_amp)."""
 
-    def __init__(self, net, B: int):
+    def __init__(self, net, B: int, amp: bool = False):
         self.net = net
+        self.amp = amp
+        self.B = B
+        if amp:
+            self._init_amp(net, B)
+            return
         dev = net._device()
         D, Wd, Te = net.input_channel, net.model_channel, net.time_emb_channel
         from .model.module import timestep_freqs
@@ -907,12 +929,136 @@ class MLPTrainer(_Generation):
         self.bwd = BP
         self.params = [p for p in net.parameters() if p.requires_grad]
 
+    def _init_amp(self, net, B: int) -> None:
+        """bf16 plans (the reference's enable_amp): every Linear except time_embed is one bf16 MMA per product with fp32
+        accumulation and fp32 output, split-K where its output tiles alone would leave SMs idle (Plan.linear_tc).  The
+        layers' linear_emb, which all read SiLU(cond), are one bank GEMM over their concatenated weights, forward and
+        backward.  Modulate, LayerNorm, SiLU and dropout write the next Linear's bf16 operand straight into a bf16 concat
+        buffer (pdae_mlp_mod_ln_act_bf16), which the weight gradient reads again; h and the bank output stay fp32 for the
+        backward, which writes fp32 and bf16 gradients in one pass (pdae_mlp_mod_ln_act_bwd_bf16).  time_embed (64 -> 512,
+        SiLU, 512 -> 512) stays fp32 on CUDA cores in the forward."""
+        dev = net._device()
+        D, Wd, Te = net.input_channel, net.model_channel, net.time_emb_channel
+        from .model.module import timestep_freqs
+        bf16 = torch.bfloat16
+        P = Plan(dev, "fp32")
+        P.keep_all = True
+        self.x_in = P.new((B, D), torch.float32, "z_t")
+        self.t_in = P.new((B,), torch.int64, "t")
+        temb = P.new((B, Te), torch.float32, "temb")
+        P.call("timestep_embedding", self.t_in, B, Te, P.fixed(timestep_freqs(Te, dev)), temb, _STREAM)
+        c0 = P.new((B, D), torch.float32, "cond_h")
+        P.linear(temb, net.time_embed[0].weight, net.time_embed[0].bias, c0, B=B, Cin=Te, Cout=D)
+        cond = P.new((B, D), torch.float32, "cond")
+        P.linear(c0, net.time_embed[2].weight, net.time_embed[2].bias, cond, B=B, Cin=D, Cout=D, a_silu=True)
+        scond = P.new((B, D), bf16, "silu_cond_bf16")     # SiLU(cond): the operand of the bank GEMM
+        P.call("mlp_mod_ln_act_bf16", cond, None, 0, None, None, F32(1e-5), 1, None, F32(1.0), scond, D, B, D, _STREAM)
+        # the bank: linear_emb of every conditioned layer, [total][D] weights / [total] bias, layer i at column offsets[i]
+        emb_layers = [layer for layer in net.layers if layer.use_cond]
+        ws, bs = [l.linear_emb.weight for l in emb_layers], [l.linear_emb.bias for l in emb_layers]
+        offsets = np.cumsum([0] + [w.shape[0] for w in ws]).tolist()
+        total = offsets[-1]
+        for p in ws + bs:
+            P.params.append((p, p.data_ptr()))
+        wbank = P.pack(("mlp_bank", id(ws[0])), ws, lambda: torch.cat([w.detach() for w in ws], 0).to(bf16))
+        bbank = P.pack(("mlp_bank_bias", id(bs[0])), bs, lambda: torch.cat([b.detach() for b in bs]).float())
+        bank = P.linear_tc(scond, wbank, bbank, B=B, Cin=D, Cout=total, name="mlp_bank")
+        x_bf = P.new((B, D), bf16, "z_t_bf16")
+        P.call("copy_cols_bf16", self.x_in, x_bf, D, 0, B, D, _STREAM)
+        cur, cin = x_bf, D
+        n = len(net.layers)
+        tape = []
+        for i, layer in enumerate(net.layers):
+            co = layer.linear.weight.shape[0]
+            w = layer.linear.weight
+            wp = P.pack((id(w), "tc"), [w], lambda w=w: w.detach().to(bf16))
+            h = P.linear_tc(cur, wp, P.param(layer.linear.bias), B=B, Cin=cin, Cout=co, name="mlp_h")
+            if i == n - 1:
+                self.out = h
+                tape.append(dict(layer=layer, x=cur, cin=cin, co=co, last=True))
+                break
+            off = offsets[emb_layers.index(layer)]
+            dst = P.new((B, Wd + D), bf16, f"cat{i}")    # one bf16 concat buffer per layer: the weight gradients read them all
+            P.call("copy_cols_bf16", self.x_in, dst, Wd + D, Wd, B, D, _STREAM)
+            ln = layer.norm if isinstance(layer.norm, nn.LayerNorm) else None
+            mask = None
+            pdrop = float(layer.dropout.p) if isinstance(layer.dropout, nn.Dropout) else 0.0
+            if net.training and pdrop > 0:
+                mask = P.new((B, co), torch.float32, "drop_mask")
+                P.dropout_masks.append((layer, mask, pdrop))
+            P.call("mlp_mod_ln_act_bf16", h, bank.at(off), total, P.param(ln.weight) if ln else None,
+                   P.param(ln.bias) if ln else None, F32(ln.eps if ln else 1e-5), 1, mask,
+                   F32(1.0 / (1.0 - pdrop) if mask is not None else 1.0), dst, Wd + D, B, co, _STREAM)
+            tape.append(dict(layer=layer, x=cur, cin=cin, co=co, last=False, h=h, off=off, ln=ln, mask=mask, pdrop=pdrop))
+            cur, cin = dst, Wd + D
+        P.finalize()
+        self.fwd = P
+
+        BP = bwd_plan(dev, amp=True)
+        self.sink = GradSink()
+        bw = Backward(BP, self.sink)
+        self.d_out = BP.new((B, D), torch.float32, "d_eps")
+        self.d_out.keep = True
+        d_bank = BP.new((B, total), torch.float32, "d_bank")        # every column block written by its layer's kernel
+        d_bank_bf = BP.new((B, total), bf16, "d_bank_bf16")
+        dy, dy_ld = self.d_out, D
+        for sv in reversed(tape):
+            layer, co, cin = sv["layer"], sv["co"], sv["cin"]
+            w = layer.linear.weight
+            if sv["last"]:
+                dh = dy
+                dh_bf = BP.new((B, co), bf16, "d_mlp_h_bf16")
+                BP.call("copy_cols_bf16", dy, dh_bf, co, 0, B, co, _STREAM)
+            else:
+                ln = sv["ln"]
+                dlw = dlb = None
+                if ln is not None:
+                    dlw, dlb = BP.new_zeroed(co), BP.new_zeroed(co)
+                    self.sink.add(ln.weight, dlw, co, lambda t: t)
+                    self.sink.add(ln.bias, dlb, co, lambda t: t)
+                dh = BP.new((B, co), torch.float32, "d_mlp_h")
+                dh_bf = BP.new((B, co), bf16, "d_mlp_h_bf16")
+                mask = sv["mask"]
+                BP.call("mlp_mod_ln_act_bwd_bf16", bw.fx(sv["h"]), bw.fx(bank).at(sv["off"]), total,
+                        BP.param(ln.weight) if ln else None, BP.param(ln.bias) if ln else None, F32(ln.eps if ln else 1e-5), 1,
+                        dy, dy_ld, bw.fx(mask), F32(1.0 / (1.0 - sv["pdrop"]) if mask is not None else 1.0), dh, dh_bf,
+                        d_bank.at(sv["off"]), d_bank_bf.at(sv["off"]), dlw, dlb, B, co, _STREAM)
+            dw = BP.new_zeroed(cin * co)
+            BP.call("wgrad_tc_bf16", bw.fx(sv["x"]), dh_bf, dw, B, 1, 1, cin, co, 1, flops=2.0 * B * cin * co)
+            self.sink.add(w, dw, cin * co, lambda t, cin=cin, co=co: t.view(cin, co).t())
+            db = BP.new_zeroed(co)
+            BP.call("colsum", dh, ctypes.c_int64(B), co, db, _STREAM)
+            self.sink.add(layer.linear.bias, db, co, lambda t: t)
+            if sv["x"] is not x_bf:                       # (no gradient w.r.t. z_t)
+                wt = BP.pack((id(w), "tc_t"), [w], lambda w=w: w.detach().t().contiguous().to(bf16))     # [cin][co]
+                dy, dy_ld = BP.linear_tc(dh_bf, wt, None, B=B, Cin=co, Cout=cin, name="d_mlp_x"), cin
+        # the bank: one weight gradient, one bias column sum, one data gradient for all conditioned layers
+        dwb = BP.new_zeroed(D * total)
+        BP.call("wgrad_tc_bf16", bw.fx(scond), d_bank_bf, dwb, B, 1, 1, D, total, 1, flops=2.0 * B * D * total)
+        dbb = BP.new_zeroed(total)
+        BP.call("colsum", d_bank, ctypes.c_int64(B), total, dbb, _STREAM)
+        for layer, off in zip(emb_layers, offsets):
+            co = layer.linear_emb.weight.shape[0]
+            self.sink.add(layer.linear_emb.weight, dwb, D * total, lambda t, off=off, co=co: t.view(D, total)[:, off:off + co].t())
+            self.sink.add(layer.linear_emb.bias, dbb, total, lambda t, off=off, co=co: t[off:off + co])
+        wbt = BP.pack(("mlp_bank_t", id(ws[0])), ws, lambda: torch.cat([w.detach() for w in ws], 0).t().contiguous().to(bf16))
+        d_scond = BP.linear_tc(d_bank_bf, wbt, None, B=B, Cin=total, Cout=D, name="d_silu_cond")
+        d_cond = BP.new((B, D), torch.float32, "d_cond")
+        BP.call("dsilu_mul", d_scond, bw.fx(cond), d_cond, ctypes.c_int64(B * D), _STREAM)
+        g = bw.conv(c0, d_cond, net.time_embed[2].weight, net.time_embed[2].bias, B=B, H=1, W=1, Cin=D, Cout=D, k=1, a_silu=True)
+        d_c0 = BP.new((B, D), torch.float32, "d_c0")
+        BP.call("dsilu_mul", g, bw.fx(c0), d_c0, ctypes.c_int64(B * D), _STREAM)
+        bw.conv(temb, d_c0, net.time_embed[0].weight, net.time_embed[0].bias, B=B, H=1, W=1, Cin=Te, Cout=D, k=1, need_dx=False)
+        BP.finalize()
+        self.bwd = BP
+        self.params = [p for p in net.parameters() if p.requires_grad]
+
     def forward(self, x, t):
         self.x_in.tensor.copy_(x)
         self.t_in.tensor.copy_(t)
         draw_dropout_masks(self.fwd)
         self.fwd.run()
-        return self.out.tensor.clone()
+        return _tensor_of(self.out, (self.B, self.net.input_channel)).clone()
 
     def backward(self, d_out):
         self.d_out.tensor.copy_(d_out)
@@ -940,9 +1086,10 @@ class _MLPFn(torch.autograd.Function):
 def mlp_train_forward(net, x, t):
     B = x.shape[0]
     cache = net.__dict__.setdefault("_train_cache", {})
-    key = (B, net.training)
+    amp = autocast_active() and mlp_amp_supported(net)
+    key = (B, net.training, amp)
     tr = cache.get(key)
     if tr is None or tr.fwd.stale() or tr.bwd.stale():
-        tr = MLPTrainer(net, B)
+        tr = MLPTrainer(net, B, amp)
         cache[key] = tr
     return _MLPFn.apply(tr, x, t, *tr.params)
