@@ -292,6 +292,13 @@ int pdae_conv_tc2_create_s2(pdae_conv_tc2_plan** plan, const void* in_bf16, cons
                             int B, int H, int W, int Cin, int Cout);
 int pdae_conv_tc2_create_s2_dgrad(pdae_conv_tc2_plan** plan, const void* dy_bf16, const void* wt_bf16, float* dx, int B, int H,
                                   int W, int Cin, int Cout);
+/* The same stride-2 forward with the stride-1 epilogue's options (the encoder's forward in the "bf16" and "bf16x3" modes):
+ * out[B][H/2][W/2][Cout] in out_dtype (PDAE_F32 or PDAE_BF16) and, if ch_stats != NULL ([B][Cout][2] fp32, 8-byte aligned,
+ * zero it first), the per-channel (sum, sum^2) of the stored values.  Cin is the operand's channel count: a split-operand
+ * input [B][H][W][hi | lo | hi] passes 3 C with weights [9][Cout][W_hi | W_hi | W_lo] for fp32-grade products.
+ * pdae_conv_tc2_create_s2 is this entry point with PDAE_F32 and no statistics.  Run / destroy as above.                 */
+int pdae_conv_tc2_create_s2_ex(pdae_conv_tc2_plan** plan, const void* in_bf16, const void* w_bf16, const float* bias, void* out,
+                               int out_dtype, float* ch_stats, int B, int H, int W, int Cin, int Cout);
 /* Split-K Linear (bf16 autocast latent training): out[B][Cout] (fp32) += in[B][Cin] (bf16) * w[Cout][Cin]^T (bf16) + bias.
  * Each output tile's k range is split so that about one wave of (tile, k range) items covers the SMs; the partial tiles are
  * added with fp32 reductions, so `out` must be zeroed before every run.  Cin, Cout multiples of 64.                     */
@@ -320,6 +327,10 @@ void pdae_conv_tc2_destroy(pdae_conv_tc2_plan* plan);
  * Cin <= 4, Cout % 8 == 0, Cout <= 256.                                                                                */
 int pdae_stem_conv_bf16(const float* x_nchw, const float* w_packed, const float* bias, void* out_bf16_nhwc, float* ch_stats,
                         int B, int H, int W, int Cin, int Cout, pdae_stream_t stream);
+/* The semantic encoder's stem, nn.Conv2d(3, 64, 3, stride 2, padding 1) (model/representation_learning/encoder/ffhq.py), the
+ * same way: H, W the input size (H even, W % 8 == 0), out_bf16_nhwc [B][H/2][W/2][Cout], arguments otherwise as above.  */
+int pdae_stem_conv_s2_bf16(const float* x_nchw, const float* w_packed, const float* bias, void* out_bf16_nhwc, float* ch_stats,
+                           int B, int H, int W, int Cin, int Cout, pdae_stream_t stream);
 
 /* ---- callers either side of the hot path (SURVEY.md 8(f)) -------------------------------------------------------------
  * Fused multi-tensor Adam + EMA: replaces torch.optim.Adam.step() as configured at

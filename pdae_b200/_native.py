@@ -107,6 +107,7 @@ _SIGS = {
     "pdae_conv_s2_tc_supported": (c_int, [c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_s2": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_s2_dgrad": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_conv_tc2_create_s2_ex": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_splitk": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, c_int, c_int]),
     "pdae_conv_tc2_run": (c_int, [_P, _P]),
     "pdae_conv_tc2_set_head_fuse": (c_int, [_P, _P]),
@@ -131,6 +132,7 @@ _SIGS = {
                                              c_int, c_int, _P]),
     "pdae_mul_mask_cols": (c_int, [_P, c_int, _P, c_float, c_int, c_int, _P]),
     "pdae_stem_conv_bf16": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "pdae_stem_conv_s2_bf16": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_gn_apply_split3": (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P]),
     "pdae_adam_ema_step": (c_int, [_P, _P, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_int64, c_float,
                                    c_float, _P]),

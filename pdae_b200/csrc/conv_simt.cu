@@ -229,7 +229,9 @@ __global__ void __launch_bounds__(256) conv3x3_smalln_kernel(const TIn* __restri
 // per-channel (sum, sum^2) of the STORED (rounded) values accumulated for the first GroupNorms (unet.py:62-64, 195).
 // HBM-bound on the output write (2 B x Cout per pixel); the image itself is tiny.  One CTA = pixels of ONE image;
 // thread -> (pixel slot, channel octet); weights [27][Cout] in shared memory.
-template <int CIN>
+// S = 2: the semantic encoder's stride-2 stem (encoder/ffhq.py: nn.Conv2d(3, 64, 3, 2, 1)); H, W stay the INPUT size and the
+// output is [B][H/2][W/2][Cout].  A thread's 4 output pixels read input columns 2 x0 - 1 .. 2 x0 + 7 of each row.
+template <int CIN, int S = 1>
 __global__ void __launch_bounds__(256) stem_conv_bf16_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                              const float* __restrict__ bias, __nv_bfloat16* __restrict__ out,
                                                              float* __restrict__ stats, int H, int W, int Cout) {
@@ -237,6 +239,7 @@ __global__ void __launch_bounds__(256) stem_conv_bf16_kernel(const float* __rest
   float* ws = sm;                          // [9*CIN][Cout]
   float* acc = sm + 9 * CIN * Cout;        // [2][Cout] per-CTA statistics
   const int b = blockIdx.y, HW = H * W;
+  const int Ho = H / S, Wo = W / S, HWo = Ho * Wo;
   for (int i = threadIdx.x; i < 9 * CIN * Cout; i += 256) ws[i] = w[i];
   for (int i = threadIdx.x; i < 2 * Cout; i += 256) acc[i] = 0.f;
   __syncthreads();
@@ -250,8 +253,8 @@ __global__ void __launch_bounds__(256) stem_conv_bf16_kernel(const float* __rest
 #pragma unroll
   for (int j = 0; j < 8; ++j) s1[j] = s2[j] = 0.f;
   const float* xb = x + (long long)b * CIN * HW;
-  const int W4 = W >> 2, nquad = H * W4;   // W % 4 == 0 (host checks): a thread owns 4 horizontally adjacent pixels,
-  if (slot < ppc) {                        // so every weight vector read from shared memory feeds 4 x 8 FMAs
+  const int W4 = Wo >> 2, nquad = Ho * W4;   // Wo % 4 == 0 (host checks): a thread owns 4 horizontally adjacent pixels,
+  if (slot < ppc) {                          // so every weight vector read from shared memory feeds 4 x 8 FMAs
     for (int qd = blockIdx.x * ppc + slot; qd < nquad; qd += gridDim.x * ppc) {
       const int y = qd / W4, x0 = (qd - y * W4) * 4;
       float a[4][8];
@@ -261,23 +264,31 @@ __global__ void __launch_bounds__(256) stem_conv_bf16_kernel(const float* __rest
         for (int j = 0; j < 8; ++j) a[pp][j] = bv[j];
 #pragma unroll
       for (int ky = 0; ky < 3; ++ky) {
-        const int iy = y + ky - 1;
+        const int iy = S * y + ky - 1;
         if (iy < 0 || iy >= H) continue;
 #pragma unroll
         for (int ci = 0; ci < CIN; ++ci) {
-          const float* row = xb + (long long)ci * HW + (long long)iy * W + x0;
-          float v[6];
-          const float4 mid = __ldg(reinterpret_cast<const float4*>(row));
-          v[0] = x0 > 0 ? __ldg(row - 1) : 0.f;
-          v[1] = mid.x; v[2] = mid.y; v[3] = mid.z; v[4] = mid.w;
-          v[5] = x0 + 4 < W ? __ldg(row + 4) : 0.f;
+          const float* row = xb + (long long)ci * HW + (long long)iy * W + S * x0;
+          float v[S == 1 ? 6 : 9];           // input columns S x0 - 1 .. S x0 + 3 S + 1
+          if constexpr (S == 1) {
+            const float4 mid = __ldg(reinterpret_cast<const float4*>(row));
+            v[0] = x0 > 0 ? __ldg(row - 1) : 0.f;
+            v[1] = mid.x; v[2] = mid.y; v[3] = mid.z; v[4] = mid.w;
+            v[5] = x0 + 4 < W ? __ldg(row + 4) : 0.f;
+          } else {                           // (the right pad column is never read: 2 (x0 + 3) + 1 <= W - 1)
+            const float4 m0 = __ldg(reinterpret_cast<const float4*>(row));
+            const float4 m1 = __ldg(reinterpret_cast<const float4*>(row + 4));
+            v[0] = x0 > 0 ? __ldg(row - 1) : 0.f;
+            v[1] = m0.x; v[2] = m0.y; v[3] = m0.z; v[4] = m0.w;
+            v[5] = m1.x; v[6] = m1.y; v[7] = m1.z; v[8] = m1.w;
+          }
 #pragma unroll
           for (int kx = 0; kx < 3; ++kx) {
             const float4 w0 = *reinterpret_cast<const float4*>(ws + ((ky * 3 + kx) * CIN + ci) * Cout + c);
             const float4 w1 = *reinterpret_cast<const float4*>(ws + ((ky * 3 + kx) * CIN + ci) * Cout + c + 4);
 #pragma unroll
             for (int pp = 0; pp < 4; ++pp) {
-              const float vv = v[pp + kx];
+              const float vv = v[S * pp + kx];
               a[pp][0] = fmaf(vv, w0.x, a[pp][0]); a[pp][1] = fmaf(vv, w0.y, a[pp][1]);
               a[pp][2] = fmaf(vv, w0.z, a[pp][2]); a[pp][3] = fmaf(vv, w0.w, a[pp][3]);
               a[pp][4] = fmaf(vv, w1.x, a[pp][4]); a[pp][5] = fmaf(vv, w1.y, a[pp][5]);
@@ -296,7 +307,7 @@ __global__ void __launch_bounds__(256) stem_conv_bf16_kernel(const float* __rest
           s1[2 * j] += r.x; s2[2 * j] = fmaf(r.x, r.x, s2[2 * j]);
           s1[2 * j + 1] += r.y; s2[2 * j + 1] = fmaf(r.y, r.y, s2[2 * j + 1]);
         }
-        *reinterpret_cast<uint4*>(out + ((long long)b * HW + (long long)y * W + x0 + pp) * Cout + c) = *reinterpret_cast<uint4*>(h);
+        *reinterpret_cast<uint4*>(out + ((long long)b * HWo + (long long)y * Wo + x0 + pp) * Cout + c) = *reinterpret_cast<uint4*>(h);
       }
     }
     if (stats) {
@@ -401,5 +412,34 @@ extern "C" int pdae_stem_conv_bf16(const float* x_nchw, const float* w_packed, c
     default: stem_conv_bf16_kernel<4><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, ch_stats, H, W, Cout); break;
   }
   PDAE_LAUNCH_CHECK("stem_conv_bf16_kernel");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_stem_conv_s2_bf16(const float* x_nchw, const float* w_packed, const float* bias, void* out_bf16_nhwc,
+                                      float* ch_stats, int B, int H, int W, int Cin, int Cout, pdae_stream_t stream) {
+  PDAE_REQUIRE(x_nchw && w_packed && out_bf16_nhwc, "stem_conv_s2_bf16: null pointer");
+  PDAE_REQUIRE(B > 0 && B <= 65535, "stem_conv_s2_bf16: B=%d must be in [1, 65535]", B);
+  PDAE_REQUIRE(Cin >= 1 && Cin <= 4, "stem_conv_s2_bf16: Cin=%d (image channels) must be 1..4", Cin);
+  PDAE_REQUIRE(Cout % 8 == 0 && Cout >= 8 && Cout <= 256, "stem_conv_s2_bf16: Cout=%d must be a multiple of 8 in [8, 256]", Cout);
+  PDAE_REQUIRE(H >= 2 && W >= 8 && H % 2 == 0 && W % 8 == 0,
+               "stem_conv_s2_bf16: H=%d W=%d: H must be even and W a multiple of 8 (4-pixel output quads)", H, W);
+  PDAE_REQUIRE(!(((uintptr_t)x_nchw | (uintptr_t)out_bf16_nhwc) & 15), "stem_conv_s2_bf16: x and out must be 16-byte aligned");
+  PDAE_REQUIRE(!((uintptr_t)ch_stats & 3), "stem_conv_s2_bf16: ch_stats must be 4-byte aligned");
+  const int Ho = H / 2, Wo = W / 2;
+  const int ppc = 256 / (Cout / 8);
+  int gx = cdiv((long long)Ho * (Wo / 4), (long long)ppc * 2);
+  if (gx > 148 * 8) gx = 148 * 8;
+  if (gx < 1) gx = 1;
+  const size_t smem = (size_t)(9 * Cin + 2) * Cout * sizeof(float);
+  dim3 grid(gx, B);
+  cudaStream_t s = (cudaStream_t)stream;
+  __nv_bfloat16* o = (__nv_bfloat16*)out_bf16_nhwc;
+  switch (Cin) {
+    case 1: stem_conv_bf16_kernel<1, 2><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, ch_stats, H, W, Cout); break;
+    case 2: stem_conv_bf16_kernel<2, 2><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, ch_stats, H, W, Cout); break;
+    case 3: stem_conv_bf16_kernel<3, 2><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, ch_stats, H, W, Cout); break;
+    default: stem_conv_bf16_kernel<4, 2><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, ch_stats, H, W, Cout); break;
+  }
+  PDAE_LAUNCH_CHECK("stem_conv_bf16_kernel<stride 2>");
   return PDAE_OK;
 }

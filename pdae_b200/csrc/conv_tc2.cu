@@ -11,12 +11,14 @@
 // The BN=16 instantiation is the UNet image head (Cout=3 zero-padded to 16): it skips the TMA store and writes the
 // first `cout_valid` columns as NCHW fp32 planes.
 //
-// S2 != 0: the three-by-three, stride-2, pad-1 convs of the semantic encoder (bf16 autocast training).  An NHWC tensor
+// S2 != 0: the three-by-three, stride-2, pad-1 convs of the semantic encoder (bf16 autocast training; the forward also in the
+// "bf16" and "bf16x3" forward-only plans).  An NHWC tensor
 // [B][H][W][C] is addressed through its PARITY VIEW, the same memory as [B][H/2][2][W/2][2C]: pixel (2 a + py, 2 b + px),
 // channel c sits at the 5-D TMA coordinate (px C + c, b, py, a, image).  Each parity class is a dense stride-1 grid.
 //   S2 = 1, forward: output row o reads input row 2 o + ky - 1 = parity (ky != 1) at row o - (ky == 0), so each tap is a box
 //           of one parity class at the output tile shifted by -1 or 0; the only out-of-range coordinate is -1, whose TMA zero
-//           fill is the padding.  The tiles cover the output grid, the epilogue is the ordinary one (bias, fp32 store).
+//           fill is the padding.  The tiles cover the output grid like the tiles of a stride-1 conv over that grid, so the
+//           epilogue is the ordinary one: bias, fp32 or bf16 store, optional per-channel statistics.
 //   S2 = 2, data gradient as four sub-pixel phases: dX at parity (py, px) is a stride-1 correlation of dY with the taps
 //           ky = 1 (py = 0) or ky = 0 at dY row + 1 and ky = 2 at dY row + 0 (py = 1), likewise kx: 1, 2, 2 or 4 taps, 9 over
 //           the four phases (the forward's MMA count).  The phase is the fastest tile index, so every CTA's contiguous tile
@@ -1165,12 +1167,25 @@ static int s2_validate(const char* fn, const void* a, const void* b, const void*
 extern "C" int pdae_conv_tc2_create_s2(pdae_conv_tc2_plan** plan_out, const void* in_bf16, const void* w_bf16, const float* bias,
                                        float* out, int B, int H, int W, int Cin, int Cout) {
   PDAE_REQUIRE(plan_out, "conv_tc2_create_s2: null pointer");
+  return pdae_conv_tc2_create_s2_ex(plan_out, in_bf16, w_bf16, bias, out, PDAE_F32, nullptr, B, H, W, Cin, Cout);
+}
+
+// The same forward with the stride-1 epilogue's options: out (fp32 or bf16 NHWC) and, optionally, the per-channel (sum, sum^2)
+// of the stored values accumulated into ch_stats [B][Cout][2].  The output grid is tiled like a stride-1 grid of H/2 x W/2, so
+// the epilogue (staging, statistics, TMA store) is the stride-1 one.  Cin is the operand's channel count: a split-operand copy
+// [hi | lo | hi] passes 3 C with [W_hi | W_hi | W_lo] weights (the parity view does not care what the 64-channel blocks mean).
+extern "C" int pdae_conv_tc2_create_s2_ex(pdae_conv_tc2_plan** plan_out, const void* in_bf16, const void* w_bf16, const float* bias,
+                                          void* out, int out_dtype, float* ch_stats, int B, int H, int W, int Cin, int Cout) {
+  PDAE_REQUIRE(plan_out, "conv_tc2_create_s2: null pointer");
   const int rc = s2_validate("conv_tc2_create_s2", in_bf16, w_bf16, out, bias, B, H, W, Cin, Cout);
   if (rc != PDAE_OK) return rc;
+  PDAE_REQUIRE(out_dtype == PDAE_F32 || out_dtype == PDAE_BF16, "conv_tc2_create_s2: bad out_dtype %d (PDAE_F32 or PDAE_BF16)",
+               out_dtype);
+  PDAE_REQUIRE(!((uintptr_t)ch_stats & 7), "conv_tc2_create_s2: ch_stats must be 8-byte aligned");
   const int Ho = H / 2, Wo = W / 2;
   Tc2Desc d;
-  d.in = in_bf16; d.w = w_bf16; d.bias = bias; d.residual = nullptr; d.out = out; d.out_dtype = PDAE_F32;
-  d.ch_stats = nullptr; d.B = B; d.H = Ho; d.W = Wo; d.Cin = Cin; d.Cout = Cout; d.ksize = 3; d.cout_valid = 0; d.bn_override = 0;
+  d.in = in_bf16; d.w = w_bf16; d.bias = bias; d.residual = nullptr; d.out = out; d.out_dtype = out_dtype;
+  d.ch_stats = ch_stats; d.B = B; d.H = Ho; d.W = Wo; d.Cin = Cin; d.Cout = Cout; d.ksize = 3; d.cout_valid = 0; d.bn_override = 0;
   d.in_ld = Cin; d.in_bs = (long long)H * W * Cin;
   d.w_batched = 0; d.w_ld = Cin; d.w_bs = (long long)Cout * Cin;
   d.out_ld = Cout; d.out_bs = (long long)Ho * Wo * Cout;
@@ -1201,8 +1216,8 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
 #define T2_GO(BN, OB) launch_tc2<BN, OB>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
-#define T2_GO_S2(BN, S2) \
-  launch_tc2<BN, false, S2>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
+#define T2_GO_S2(BN, OB, S2) \
+  launch_tc2<BN, OB, S2>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
 #define T2_GO_GM(BN, OB, GM) \
   launch_tc2<BN, OB, 0, GM>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
   const bool ob = pl->args.out_bf16 != 0;
@@ -1213,8 +1228,9 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
   else if (pl->gm == GM_B_MN) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_B_MN) : T2_GO_GM(64, false, GM_B_MN);
   else if (pl->gm == (GM_A_MN | GM_B_MN))
     e = pl->BN == 128 ? T2_GO_GM(128, false, GM_A_MN | GM_B_MN) : T2_GO_GM(64, false, GM_A_MN | GM_B_MN);
-  else if (pl->s2 == 1) e = pl->BN == 128 ? T2_GO_S2(128, 1) : T2_GO_S2(64, 1);
-  else if (pl->s2 == 2) e = pl->BN == 128 ? T2_GO_S2(128, 2) : T2_GO_S2(64, 2);
+  else if (pl->s2 == 1 && ob) e = pl->BN == 128 ? T2_GO_S2(128, true, 1) : T2_GO_S2(64, true, 1);
+  else if (pl->s2 == 1) e = pl->BN == 128 ? T2_GO_S2(128, false, 1) : T2_GO_S2(64, false, 1);
+  else if (pl->s2 == 2) e = pl->BN == 128 ? T2_GO_S2(128, false, 2) : T2_GO_S2(64, false, 2);
   else switch (pl->BN) {
     case 16: e = T2_GO(16, false); break;
     case 64: e = ob ? T2_GO(64, true) : T2_GO(64, false); break;

@@ -409,18 +409,19 @@ class Plan:
         return (self.L.pdae_wgrad_tc_run, [h, None], 1, "wgrad_tc" if split else "wgrad_tc_bf16")
 
     def _compile_s2(self, fn, args):
-        """3x3 stride-2 convs of a bf16 training step: forward (a = bf16 input, b = [9][Cout][Cin] weights, c = fp32 output),
-        data gradient (a = bf16 dy, b = [9][Cin][Cout] weights, c = fp32 dx), weight gradient (a = bf16 input, b = bf16 dy,
-        c = fp32 dw).  H, W: the conv's input size."""
+        """3x3 stride-2 convs: forward (a = bf16 or split-operand input, b = [9][Cout][Cin] weights, c = fp32 or bf16 output,
+        optional statistics), data gradient (a = bf16 dy, b = [9][Cin][Cout] weights, c = fp32 dx), weight gradient
+        (a = bf16 input, b = bf16 dy, c = fp32 dw).  H, W: the conv's input size."""
         h = ctypes.c_void_p()
         if fn == "conv_tc2_s2":
-            a, b, bias, c, B, H, W, Cin, Cout = args
-            create, extra = self.L.pdae_conv_tc2_create_s2, [self._resolve(bias)]
+            a, b, bias, c, odt, stats, B, H, W, Cin, Cout = args
+            create = self.L.pdae_conv_tc2_create_s2_ex
+            rc = create(ctypes.byref(h), self._resolve(a), self._resolve(b), self._resolve(bias), self._resolve(c), odt,
+                        self._resolve(stats), B, H, W, Cin, Cout)
         else:
             a, b, c, B, H, W, Cin, Cout = args
             create = self.L.pdae_conv_tc2_create_s2_dgrad if fn == "conv_tc2_s2_dgrad" else self.L.pdae_wgrad_tc_create_bf16_s2
-            extra = []
-        rc = create(ctypes.byref(h), self._resolve(a), self._resolve(b), *extra, self._resolve(c), B, H, W, Cin, Cout)
+            rc = create(ctypes.byref(h), self._resolve(a), self._resolve(b), self._resolve(c), B, H, W, Cin, Cout)
         _native.check(rc, create.__name__)
         if fn == "wgrad_tc_bf16_s2":
             self._wg_handles.append(h)
@@ -624,6 +625,11 @@ class Plan:
     def use_tc(self, Cin: int, Cout: int, k: int, stride: int, H: int, W: int) -> bool:
         return self.tc and self._tc_shape_ok(Cin, Cout, k, stride, H, W)
 
+    def can_conv_s2(self, H: int, W: int, Cin: int, Cout: int) -> bool:
+        """Does a forward-only plan run a 3x3 stride-2 pad-1 conv of an H x W input on the tensor cores (Plan.conv, with a bf16
+        or split-operand input)?  Training forward plans keep their own rules (train_tc)."""
+        return self.tc and self.train_tc is None and bool(self.L.pdae_conv_s2_tc_supported(H, W, Cin, Cout))
+
     def _tc_shape_ok(self, Cin: int, Cout: int, k: int, stride: int, H: int, W: int) -> bool:
         if stride != 1 or k not in (1, 3) or Cin % 64 or Cout % 64:
             return False
@@ -664,9 +670,25 @@ class Plan:
             wp = self.pack((wkey or id(weight), "tc"), [weight],
                            lambda: weight.detach().reshape(Cout, Cin, 9).permute(2, 0, 1).to(torch.bfloat16))
             x.tc_copy = xt
-            self.call("conv_tc2_s2", xt, wp, self.param(bias), out, B, H, W, Cin, Cout,
+            self.call("conv_tc2_s2", xt, wp, self.param(bias), out, PDAE_F32, None, B, H, W, Cin, Cout,
                       flops=2.0 * B * (H // 2) * (W // 2) * Cout * Cin * 9)
             return None
+        if (self.train_tc is None and stride == 2 and k == 3 and pad == 1 and x.dtype == torch.bfloat16
+                and not (in_nchw or out_nchw or a_silu) and skip is None and w_transform is None and residual is None
+                and self.can_conv_s2(H, W, Cin, Cout)):
+            # forward-only 3x3 stride-2 conv in a tensor-core mode (the semantic encoder): conv_tc2 reads the bf16 activation
+            # ("bf16") or its [hi | lo | hi] split copy ("bf16x3") through its parity view; the epilogue writes the output in its
+            # dtype and, on request, the per-channel statistics of the stored values
+            if x.split3:
+                wp = self.pack((wkey or id(weight), "tc_x3"), [weight],
+                               lambda Cin=Cin: split3_weights(weight.detach().reshape(Cout, Cin, 9)))
+            else:
+                wp = self.pack((wkey or id(weight), "tc"), [weight],
+                               lambda: weight.detach().reshape(Cout, Cin, 9).permute(2, 0, 1).to(torch.bfloat16))
+            stats = self.new_stats(B, Cout) if want_stats else None
+            self.call("conv_tc2_s2", x, wp, self.param(bias), out, _DT[out.dtype], stats, B, H, W, 3 * Cin if x.split3 else Cin,
+                      Cout, flops=2.0 * B * (H // 2) * (W // 2) * Cout * Cin * 9)
+            return stats
         if (self.train_tc and x.dtype == torch.float32 and out.dtype == torch.float32 and not (in_nchw or out_nchw or a_silu)
                 and skip is None and w_transform is None and pad == k // 2 and self._tc_shape_ok(Cin, Cout, k, stride, H, W)):
             if self.train_tc == "bf16x3":
@@ -808,19 +830,26 @@ class Plan:
         self.call("conv2d_simt", x, PDAE_F32, 0, wp, bias, None, out, 0, B, 1, 1, Cin, Cout, 1, 1, 0, int(a_silu), _STREAM,
                   flops=2.0 * B * Cin * Cout)
 
-    def linear_tc(self, x, wp: Buf, bias: Optional[Buf], *, B, Cin, Cout, name="linear_tc"):
+    def linear_tc(self, x, wp: Buf, bias: Optional[Buf], *, B, Cin, Cout, name="linear_tc", out: Optional[Buf] = None,
+                  flops: Optional[float] = None):
         """out[B][Cout] (fp32) = x[B][Cin] (bf16) wp[Cout][Cin]^T (bf16) + bias, one bf16 MMA per product on conv_tc2; returns
         out.  When the output tiles alone would leave SMs idle (the latent MLP's Linears at training batch sizes: one 128-row
         tile row) it runs split-K (pdae_conv_tc2_create_splitk): out is then a slice of the plan's zeroed arena, which the
-        plan's leading pdae_zero op clears on every replay, and the partial tiles are added into it."""
+        plan's leading pdae_zero op clears on every replay, and the partial tiles are added into it.
+        out: a given fp32 [B][Cout] buffer (e.g. a plan output) to write instead; under split-K a pdae_zero op clears it first.
+        flops: the algorithmic FLOPs to record (a split-operand x / wp hold three bf16 blocks per logical channel)."""
         assert Cin % 64 == 0 and Cout % 64 == 0, (Cin, Cout)
-        fl = 2.0 * B * Cin * Cout
+        fl = 2.0 * B * Cin * Cout if flops is None else flops
         tiles = -(-B // 128) * (Cout // (128 if Cout % 128 == 0 else 64))   # = conv_tc2's output tiles
         if tiles < torch.cuda.get_device_properties(self.device).multi_processor_count:
-            out = self.new_zeroed(B * Cout)
+            if out is None:
+                out = self.new_zeroed(B * Cout)
+            else:
+                self.call("zero", out, ctypes.c_int64(B * Cout * 4), _STREAM)
             self.call("conv_tc2_splitk", x, wp, bias, out, B, Cin, Cout, flops=fl)
             return out
-        out = self.new((B, Cout), torch.float32, name)
+        if out is None:
+            out = self.new((B, Cout), torch.float32, name)
         self.call("conv_tc2", x, wp, bias, None, out, PDAE_F32, None, B, 1, 1, Cin, Cout, 1, 0, 0, flops=fl)
         return out
 

@@ -11,7 +11,7 @@ from typing import List
 import torch
 import torch.nn as nn
 
-from ....engine import Plan, RESAMPLE_NONE
+from ....engine import _STREAM, Plan, RESAMPLE_NONE
 from ...module import AttentionBlock, PlannedModule, Slots, Src, normalization
 
 
@@ -45,6 +45,11 @@ class ConvStackEncoder(PlannedModule):
         self.encoder = Slots(slots)
 
     def _build(self, P: Plan, B: int, H: int, W: int):
+        """The forward-only plan.  "fp32": every conv and the Linear on the CUDA cores.  "bf16" / "bf16x3": the stride-2 convs
+        after the stem on the tensor cores (conv_tc2 through parity views) on the bf16 / split-operand GroupNorm-SiLU output,
+        writing the stream dtype and the next GroupNorm's statistics; the final Linear as a bf16 / split-operand GEMM.  The
+        stem computes in fp32 on the CUDA cores either way: the stride-2 stem kernel writing the bf16 stream and its statistics
+        in "bf16", the fp32 conv in "bf16x3"."""
         x_in = P.new((B, 3, H, W), torch.float32, "x_nchw")
         x_in.keep = True
         h = None
@@ -56,30 +61,69 @@ class ConvStackEncoder(PlannedModule):
             if kind == "conv":
                 Co = m.weight.shape[0]
                 Ho, Wo = H // 2, W // 2
-                out = P.new((B, Ho, Wo, Co), torch.float32, "enc_h")
                 if h is None:
-                    P.conv(x_in, m.weight, m.bias, out, B=B, H=H, W=W, Cin=3, Cout=Co, k=3, stride=2, pad=1, in_nchw=True)
+                    h = self._emit_stem(P, m, x_in, B, H, W)
                 else:
+                    tc = P.can_conv_s2(H, W, C, Co)
                     act, _ = P.gn_apply(h.b1, C, None, 0, pending_ab, silu=True, resample=RESAMPLE_NONE, B=B, H=H, W=W,
-                                        act_dtype=torch.float32)
-                    P.conv(act, m.weight, m.bias, out, B=B, H=H, W=W, Cin=C, Cout=Co, k=3, stride=2, pad=1)
-                h, C, H, W = Src(out, Co, B, Ho, Wo), Co, Ho, Wo
+                                        act_dtype=torch.bfloat16 if tc else torch.float32)
+                    out = P.new((B, Ho, Wo, Co), P.stream_dtype if tc else torch.float32, "enc_h")
+                    st = P.conv(act, m.weight, m.bias, out, B=B, H=H, W=W, Cin=C, Cout=Co, k=3, stride=2, pad=1,
+                                want_stats=tc)
+                    h = Src(out, Co, B, Ho, Wo, s1=st)
+                C, H, W = Co, Ho, Wo
             elif kind == "gn":
-                pending_ab = P.gn_coef(h.b1, C, None, 0, m.weight, m.bias, B=B, HW=H * W)
+                pending_ab = P.gn_coef(h.b1, C, None, 0, m.weight, m.bias, B=B, HW=H * W, stats1=h.s1)
             elif kind == "attn":
                 h = m.emit(P, h)
             else:  # final GN+SiLU, View(-1, C*4*4) in NCHW order, Linear
-                act, _ = P.gn_apply(h.b1, C, None, 0, pending_ab, silu=True, resample=RESAMPLE_NONE, B=B, H=H, W=W,
-                                    act_dtype=torch.float32)
-                # the reference flattens NCHW (c, y, x); our activation is NHWC (y, x, c): permute the weight instead
-                wt = m.weight
-                HW = H * W
-                wp = P.pack((id(wt), "enc_fc"), [wt],
-                            lambda: wt.detach().reshape(-1, C, HW).permute(2, 1, 0).reshape(HW * C, -1).float())
                 z = P.new((B, self.latent_dim), torch.float32, "z")
                 z.keep = True
-                P.linear_packed(act, wp, P.param(m.bias), z, B=B, Cin=HW * C, Cout=self.latent_dim)
+                self._emit_linear(P, m, h, pending_ab, z, B, H, W, C)
         return x_in, z
+
+    def _emit_stem(self, P: Plan, m: nn.Conv2d, x_in, B: int, H: int, W: int) -> Src:
+        Co = m.weight.shape[0]
+        Ho, Wo = H // 2, W // 2
+        if P.stream_bf16 and Co % 8 == 0 and Co <= 256 and W % 8 == 0:
+            # bf16 stream from the first layer: the stride-2 stem writes bf16 NHWC and the first GroupNorm's statistics
+            wt = m.weight
+            wp = P.pack((id(wt), "stem"), [wt], lambda: wt.detach().reshape(Co, 3, 9).permute(2, 1, 0).float())   # [9][Cin][Cout]
+            out = P.new((B, Ho, Wo, Co), torch.bfloat16, "enc_stem")
+            st = P.new_stats(B, Co)
+            P.call("stem_conv_s2_bf16", x_in, wp, P.param(m.bias), out, st, B, H, W, 3, Co, _STREAM,
+                   flops=2.0 * B * Ho * Wo * Co * 3 * 9)
+            return Src(out, Co, B, Ho, Wo, s1=st)
+        out = P.new((B, Ho, Wo, Co), torch.float32, "enc_h")
+        P.conv(x_in, m.weight, m.bias, out, B=B, H=H, W=W, Cin=3, Cout=Co, k=3, stride=2, pad=1, in_nchw=True)
+        return Src(out, Co, B, Ho, Wo)
+
+    def _emit_linear(self, P: Plan, m: nn.Linear, h: Src, pending_ab, z, B: int, H: int, W: int, C: int) -> None:
+        # the reference flattens NCHW (c, y, x); our activation is NHWC (y, x, c): permute the weight instead
+        wt = m.weight
+        HW, D = H * W, self.latent_dim
+        tc = P.tc and D % 64 == 0 and (HW * C) % 64 == 0
+        act, _ = P.gn_apply(h.b1, C, None, 0, pending_ab, silu=True, resample=RESAMPLE_NONE, B=B, H=H, W=W,
+                            act_dtype=torch.bfloat16 if tc else torch.float32)
+        if not tc:
+            wp = P.pack((id(wt), "enc_fc"), [wt],
+                        lambda: wt.detach().reshape(-1, C, HW).permute(2, 1, 0).reshape(HW * C, -1).float())
+            P.linear_packed(act, wp, P.param(m.bias), z, B=B, Cin=HW * C, Cout=D)
+            return
+        if P.x3:
+            # per pixel [W_hi | W_hi | W_lo] against the activation's [a_hi | a_lo | a_hi] blocks: K = 3 HW C
+            def pack_x3():
+                w = wt.detach().reshape(D, C, HW).permute(0, 2, 1).float()          # [D][HW][C]
+                hi = w.to(torch.bfloat16)
+                lo = (w - hi.float()).to(torch.bfloat16)
+                return torch.cat([hi, hi, lo], dim=2).reshape(D, 3 * HW * C)
+            wp = P.pack((id(wt), "enc_fc_x3"), [wt], pack_x3)
+            K = 3 * HW * C
+        else:
+            wp = P.pack((id(wt), "enc_fc_tc"), [wt],
+                        lambda: wt.detach().reshape(D, C, HW).permute(0, 2, 1).reshape(D, HW * C).to(torch.bfloat16))
+            K = HW * C
+        P.linear_tc(act, wp, P.param(m.bias), B=B, Cin=K, Cout=D, out=z, flops=2.0 * B * HW * C * D)
 
     def forward(self, x):
         """x [N,3,S,S] fp32 -> z [N, latent_dim]."""
