@@ -129,6 +129,17 @@ int pdae_q_sample(const float* x0, const float* noise, const int64_t* t, const f
 int pdae_noise_p_sample(const float* x, const float* eps, const float* noise, const float* learned_range,
                         const int64_t* t, const float* tab_cx, const float* tab_ce, const float* tab_logvar,
                         const float* tab_logbeta, float* out, int B, int64_t per_sample, pdae_stream_t stream);
+/* pdae_noise_p_sample on a network's raw outputs (gaussian_diffusion.py:216-229, :257-270): eps and learned_range are read
+ * at per-sample stride eps_ld (>= per_sample; 2*per_sample with learned_range = eps + per_sample: the two halves of a
+ * learned-sigma output); with grad (optional, then tab_shift = shift_coef) the epsilon is eps + shift[t]*grad, one rounding
+ * after the product and one after the sum.  out may alias x.                                          */
+int pdae_noise_p_sample_shift(const float* x, const float* eps, const float* grad, const float* tab_shift, const float* noise,
+                              const float* learned_range, int64_t eps_ld, const int64_t* t, const float* tab_cx,
+                              const float* tab_ce, const float* tab_logvar, const float* tab_logbeta, float* out, int B,
+                              int64_t per_sample, pdae_stream_t stream);
+/* ddim.py:168 trajectory-interpolation gradient: out = ab[0]*g1 + ab[1]*g2 (fp32, one rounding per product and sum), with
+ * ab = { fp32(1 - alpha), fp32(alpha) } in DEVICE memory.  out may alias g1 or g2.                      */
+int pdae_grad_blend(const float* g1, const float* g2, const float* ab, float* out, int64_t n, pdae_stream_t stream);
 
 /* ---- latent MLP row op (mlp_skip_net.py:123-141) -------------------------------------------------
  * y = act( LN( h * (1 + cond) ) ) per row; cond/ln_w optional; act = SiLU if silu.  out has row stride
@@ -305,9 +316,14 @@ int pdae_conv_tc2_create_s2_ex(pdae_conv_tc2_plan** plan, const void* in_bf16, c
 int pdae_conv_tc2_create_splitk(pdae_conv_tc2_plan** plan, const void* in_bf16, const void* w_bf16, const float* bias, float* out,
                                 int B, int Cin, int Cout);
 int pdae_conv_tc2_run(const pdae_conv_tc2_plan* plan, pdae_stream_t stream);
-/* Image-head plans (cout_valid > 0): fuse the per-step DDIM update (diffusion/ddim.py:43-55,66-79,91-107,123-138) into the head's
- * epilogue.  fuse_desc_device: 8 x int64 in DEVICE memory, read at run time = { flags, eps*, x_t*, t*, tab_A*, tab_Bm*, tab_s1m*,
- * tab_ab* }, flags = enabled | use_grad<<1 | eps_only<<2 | C<<8 | C_eps<<16; flags == 0 -> plain head.  Arithmetic identical to pdae_ddim_step. */
+/* Image-head plans (cout_valid > 0): fuse the per-step sampling update into the head's epilogue, x_t updated in place.
+ * fuse_desc_device: 10 x int64 in DEVICE memory, read at run time, flags = enabled | use_grad<<1 | eps_only<<2 | ddpm<<3 |
+ * interp<<4 | C<<8 | C_eps<<16; flags == 0 -> plain head.
+ *  DDIM (diffusion/ddim.py:43-55,66-79,91-107,123-138): { flags, eps*, x_t*, t*, tab_A*, tab_Bm*, tab_s1m*, tab_ab*, g1*, a };
+ *    arithmetic identical to pdae_ddim_step.  interp (ddim.py:149-174, on the second shift head, with use_grad): the gradient is
+ *    a1*g1 + a2*head with a = fp32 bits of a1 = 1 - alpha in the low and of a2 = alpha in the high 32 bits (pdae_grad_blend).
+ *  ddpm (gaussian_diffusion.py:112-126): { flags, eps*, x_t*, t*, tab_cx*, tab_ce*, tab_shift*, tab_logvar*, noise*, 0 };
+ *    arithmetic identical to pdae_noise_p_sample_shift (use_grad: eps + shift[t] * head) or pdae_noise_p_sample.               */
 int pdae_conv_tc2_set_head_fuse(pdae_conv_tc2_plan* plan, const int64_t* fuse_desc_device);
 /* P = softmax(alpha * S) per row, fp32 in -> bf16 out.  vT[b*heads+h][c][t] = V part of qkv (bf16 [B][T][3C]).        */
 int pdae_softmax_bf16(const float* S, void* P_bf16, int64_t rows, int cols, float alpha, pdae_stream_t stream);

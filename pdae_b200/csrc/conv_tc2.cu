@@ -432,19 +432,42 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               const float* eps = reinterpret_cast<const float*>(__ldg(p.fuse + 1));
               float* xt = reinterpret_cast<float*>(__ldg(p.fuse + 2));
               const long long tb = reinterpret_cast<const long long*>(__ldg(p.fuse + 3))[b];
-              const float A = reinterpret_cast<const float*>(__ldg(p.fuse + 4))[tb];
-              const float Bm = reinterpret_cast<const float*>(__ldg(p.fuse + 5))[tb];
-              const float abar = reinterpret_cast<const float*>(__ldg(p.fuse + 7))[tb];
-              const float s1m = (flags & 2) ? reinterpret_cast<const float*>(__ldg(p.fuse + 6))[tb] : 0.f;
               const long long xi = ((long long)b * C + j) * hw + pix;
-              float e = val;                                  // this head predicts epsilon itself
-              if (flags & 2) e = __fsub_rn(eps[((long long)b * Ce + j) * hw + pix], __fmul_rn(s1m, val));   // own output = shift term
-              else if (flags & 4) e = eps[((long long)b * Ce + j) * hw + pix];   // shift unused this step: epsilon from the other head
-              const float ax = __fmul_rn(A, xt[xi]);
-              float x0v = __fsub_rn(ax, __fmul_rn(Bm, e));
-              x0v = fminf(fmaxf(x0v, -1.0f), 1.0f);
-              const float e2 = __fdiv_rn(__fsub_rn(ax, x0v), Bm);
-              xt[xi] = __fadd_rn(__fmul_rn(x0v, sqrtf(abar)), __fmul_rn(sqrtf(__fsub_rn(1.0f, abar)), e2));
+              if (flags & 8) {
+                // DDPM ancestral step (gaussian_diffusion.py:112-126), the arithmetic of noise_p_sample_kernel; the grad head adds
+                // the shift term first as the reference does (eps + shift_coef[t] * grad, one rounding each).
+                const float* tab = reinterpret_cast<const float*>(__ldg(p.fuse + 4));
+                float e = val;
+                if (flags & 2) e = __fadd_rn(eps[((long long)b * Ce + j) * hw + pix],
+                                             __fmul_rn(reinterpret_cast<const float*>(__ldg(p.fuse + 6))[tb], val));
+                const float mean = __fsub_rn(__fmul_rn(tab[tb], xt[xi]),
+                                             __fmul_rn(reinterpret_cast<const float*>(__ldg(p.fuse + 5))[tb], e));
+                const float lv = reinterpret_cast<const float*>(__ldg(p.fuse + 7))[tb];
+                const float mask = tb == 0 ? 0.0f : 1.0f;
+                const float nz = reinterpret_cast<const float*>(__ldg(p.fuse + 8))[xi];
+                xt[xi] = __fadd_rn(mean, __fmul_rn(__fmul_rn(mask, expf(__fmul_rn(0.5f, lv))), nz));
+              } else {
+                const float A = reinterpret_cast<const float*>(__ldg(p.fuse + 4))[tb];
+                const float Bm = reinterpret_cast<const float*>(__ldg(p.fuse + 5))[tb];
+                const float abar = reinterpret_cast<const float*>(__ldg(p.fuse + 7))[tb];
+                const float s1m = (flags & 2) ? reinterpret_cast<const float*>(__ldg(p.fuse + 6))[tb] : 0.f;
+                float g = val;
+                if (flags & 16) {
+                  // trajectory interpolation (ddim.py:149-174): this is the second shift head; the first one wrote g1.  The
+                  // blend is (1 - alpha) * g1 + alpha * g2 as torch evaluates it in fp32: a1 = fp32(1 - alpha), a2 = fp32(alpha).
+                  const unsigned long long ab = (unsigned long long)__ldg(p.fuse + 9);
+                  const float a1 = __uint_as_float((unsigned)ab), a2 = __uint_as_float((unsigned)(ab >> 32));
+                  g = __fadd_rn(__fmul_rn(a1, reinterpret_cast<const float*>(__ldg(p.fuse + 8))[xi]), __fmul_rn(a2, val));
+                }
+                float e = val;                                  // this head predicts epsilon itself
+                if (flags & 2) e = __fsub_rn(eps[((long long)b * Ce + j) * hw + pix], __fmul_rn(s1m, g));   // own output = shift term
+                else if (flags & 4) e = eps[((long long)b * Ce + j) * hw + pix];   // shift unused this step: epsilon from the other head
+                const float ax = __fmul_rn(A, xt[xi]);
+                float x0v = __fsub_rn(ax, __fmul_rn(Bm, e));
+                x0v = fminf(fmaxf(x0v, -1.0f), 1.0f);
+                const float e2 = __fdiv_rn(__fsub_rn(ax, x0v), Bm);
+                xt[xi] = __fadd_rn(__fmul_rn(x0v, sqrtf(abar)), __fmul_rn(sqrtf(__fsub_rn(1.0f, abar)), e2));
+              }
             }
           }
         }
@@ -1248,10 +1271,13 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
   return PDAE_OK;
 }
 
-// Image-head plans only: attach the device-side descriptor of the fused DDIM update, 8 x int64 =
-// { flags, eps*, x_t*, t*, sqrt_recip_alphas_cumprod*, sqrt_recip_alphas_cumprod_m1*, sqrt_one_minus_alphas_cumprod*, alphas_cumprod_prev|next* }
-// with flags = enabled | use_grad << 1 | eps_only << 2 | C << 8 | C_eps << 16.  The head keeps writing its own output; when enabled it also
-// updates x_t in place (use_grad: this head produces the shift/gradient term and `eps` comes from the other head).
+// Image-head plans only: attach the device-side descriptor of the fused sampling update, 10 x int64 =
+// { flags, eps*, x_t*, t*, sqrt_recip_alphas_cumprod*, sqrt_recip_alphas_cumprod_m1*, sqrt_one_minus_alphas_cumprod*, alphas_cumprod_prev|next*,
+//   g1*, fp32 bits of (1 - alpha) | fp32 bits of alpha << 32 }
+// with flags = enabled | use_grad << 1 | eps_only << 2 | ddpm << 3 | interp << 4 | C << 8 | C_eps << 16.  The head keeps writing its own output;
+// when enabled it also updates x_t in place (use_grad: this head produces the shift/gradient term and `eps` comes from the other head;
+// interp: the gradient is the alpha-blend of g1 and this head's output).  ddpm: the DDPM ancestral step instead, with slots 4..8 =
+// { noise_posterior_mean_x_t_coef*, noise_posterior_mean_noise_coef*, shift_coef*, posterior_log_variance_clipped*, noise* }.
 extern "C" int pdae_conv_tc2_set_head_fuse(pdae_conv_tc2_plan* pl, const int64_t* fuse_desc_device) {
   PDAE_REQUIRE(pl && pl->BN == 16, "conv_tc2_set_head_fuse: not an image-head plan");
   pl->args.fuse = reinterpret_cast<const long long*>(fuse_desc_device);

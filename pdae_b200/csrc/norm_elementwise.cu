@@ -541,6 +541,42 @@ __global__ void noise_p_sample_kernel(const float* __restrict__ x, const float* 
   }
 }
 
+// noise_p_sample_kernel with eps (and lr) read at per-sample stride eps_ld (the two halves of a learned-sigma output) and an
+// optional shift term added first: e = eps + shift[t] * grad, rounded after the product and after the sum like the reference.
+__global__ void noise_p_sample_shift_kernel(const float* __restrict__ x, const float* __restrict__ eps,
+                                            const float* __restrict__ grad, const float* __restrict__ tS,
+                                            const float* __restrict__ noise, const float* __restrict__ lr, long long eps_ld,
+                                            const int64_t* __restrict__ t, const float* __restrict__ cx,
+                                            const float* __restrict__ ce, const float* __restrict__ logvar,
+                                            const float* __restrict__ logbeta, float* __restrict__ out,
+                                            long long per_sample, long long total) {
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < total;
+       i += (long long)gridDim.x * blockDim.x) {
+    const long long b = i / per_sample;
+    const long long ei = b * eps_ld + (i - b * per_sample);
+    const int64_t tb = t[b];
+    float e = eps[ei];
+    if (grad) e = __fadd_rn(e, __fmul_rn(tS[tb], grad[i]));
+    const float mean = __fsub_rn(__fmul_rn(cx[tb], x[i]), __fmul_rn(ce[tb], e));
+    float lv = logvar[tb];
+    if (lr) {
+      const float frac = __fmul_rn(__fadd_rn(lr[ei], 1.0f), 0.5f);
+      lv = __fadd_rn(lv, __fmul_rn(frac, __fsub_rn(logbeta[tb], lv)));
+    }
+    const float mask = tb == 0 ? 0.0f : 1.0f;
+    out[i] = __fadd_rn(mean, __fmul_rn(__fmul_rn(mask, expf(__fmul_rn(0.5f, lv))), noise[i]));
+  }
+}
+
+// (1 - alpha) * g1 + alpha * g2 in fp32 as torch evaluates it: ab = { fp32(1 - alpha), fp32(alpha) } in device memory, so a
+// captured step graph serves every alpha.
+__global__ void grad_blend_kernel(const float* __restrict__ g1, const float* __restrict__ g2, const float* __restrict__ ab,
+                                  float* __restrict__ out, long long n) {
+  const float a1 = ab[0], a2 = ab[1];
+  for (long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x)
+    out[i] = __fadd_rn(__fmul_rn(a1, g1[i]), __fmul_rn(a2, g2[i]));
+}
+
 // one CTA per row: y = act(LN(h*(1+cond))) (* mask * scale, the inverted dropout of pdae_mul_mask_cols); cond row b at
 // cond + b * cond_ld.  OutT = float: pdae_mlp_mod_ln_act.  OutT = bf16: the next Linear's tensor-core operand, bf16_rn of
 // exactly the fp32 value (same reduction order, same expressions).
@@ -847,6 +883,29 @@ extern "C" int pdae_noise_p_sample(const float* x, const float* eps, const float
   noise_p_sample_kernel<<<ew_grid(total), 256, 0, (cudaStream_t)stream>>>(x, eps, noise, learned_range, t, tab_cx, tab_ce,
                                                                          tab_logvar, tab_logbeta, out, per_sample, total);
   PDAE_LAUNCH_CHECK("noise_p_sample_kernel");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_noise_p_sample_shift(const float* x, const float* eps, const float* grad, const float* tab_shift,
+                                         const float* noise, const float* learned_range, int64_t eps_ld, const int64_t* t,
+                                         const float* tab_cx, const float* tab_ce, const float* tab_logvar,
+                                         const float* tab_logbeta, float* out, int B, int64_t per_sample,
+                                         pdae_stream_t stream) {
+  PDAE_REQUIRE(x && eps && noise && t && tab_cx && tab_ce && tab_logvar && out, "noise_p_sample_shift: null pointer");
+  PDAE_REQUIRE(!grad || tab_shift, "noise_p_sample_shift: grad given without shift_coef table");
+  PDAE_REQUIRE(!learned_range || tab_logbeta, "noise_p_sample_shift: learned_range needs log(betas)");
+  PDAE_REQUIRE(eps_ld >= per_sample, "noise_p_sample_shift: eps_ld < per_sample");
+  const long long total = (long long)B * per_sample;
+  noise_p_sample_shift_kernel<<<ew_grid(total), 256, 0, (cudaStream_t)stream>>>(
+      x, eps, grad, tab_shift, noise, learned_range, eps_ld, t, tab_cx, tab_ce, tab_logvar, tab_logbeta, out, per_sample, total);
+  PDAE_LAUNCH_CHECK("noise_p_sample_shift_kernel");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_grad_blend(const float* g1, const float* g2, const float* ab, float* out, int64_t n, pdae_stream_t stream) {
+  PDAE_REQUIRE(g1 && g2 && ab && out && n > 0, "grad_blend: bad args");
+  grad_blend_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(g1, g2, ab, out, n);
+  PDAE_LAUNCH_CHECK("grad_blend_kernel");
   return PDAE_OK;
 }
 

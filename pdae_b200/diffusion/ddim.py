@@ -14,6 +14,7 @@ import numpy as np
 import torch
 
 from .. import _native
+from ..engine import FUSE_DESC_LEN
 
 
 def _ptr(t):
@@ -37,24 +38,34 @@ def _t64(t, B, what):
     return t
 
 
+def graphable(net, x) -> bool:
+    """Does a sampling loop over `net` run on the one-graph-per-step path (a pdae_b200 UNet / ShiftUNet on a 4-D CUDA input
+    with autograd off)?  Any other callable takes the generic per-step loop."""
+    from ..model.shift_unet import ShiftUNet
+    from ..model.unet import UNet
+    return isinstance(net, (ShiftUNet, UNet)) and x.is_cuda and x.dim() == 4 and not torch.is_grad_enabled()
+
+
 class _StepRunner:
     """One network plan + the loop bookkeeping + the fused update of a DDIM loop direction, replayed as ONE CUDA graph per
-    step.  The graph is cached on the plan, keyed by (DDIM object, direction, shift) -- those fix the table pointers the
-    update kernel reads.  `seek(i)` sets the device-side step counter; `step()` is a single graph launch."""
+    step.  The graph is cached on the plan, keyed by (owner, kind, shift) -- those fix the table pointers the update
+    reads; the cache entry keeps the owner (DDIM / GaussianDiffusion object) alive so its id is not reused.  `seek(i)` sets
+    the device-side step counter; `step()` is a single graph launch.  _DDPMRunner and _InterpRunner change the update."""
 
-    def __init__(self, ddim: "DDIM", plan, x_in, t_in, eps, grad, direction: str, C: int):
+    def __init__(self, ddim, plan, x_in, t_in, eps, grad, direction: str, C: int, tmap=None, key=None):
         self.d, self.plan, self.x_in, self.t_in, self.eps, self.grad, self.direction = ddim, plan, x_in, t_in, eps, grad, direction
+        self.tmap = ddim.timestep_map if tmap is None else tmap
         dev = ddim.device
         B = x_in.tensor.shape[0]
         self.B = B
-        self.delta = -1 if direction == "sample" else 1
+        self.delta = 1 if direction == "encode" else -1
         # the update runs inside the step graph (separate kernel, or fused into the last head conv's epilogue); only a learn_sigma
         # head on the CUDA-core path (2C output channels, no fusable epilogue) needs it after the replay
         self.in_graph_update = eps.tensor.shape[1] == C or bool(getattr(plan, "head_fuse", None))
         self.fused = False
         self.C = C
         cache = plan.__dict__.setdefault("_step_cache", {})
-        key = (id(ddim), direction, grad is not None)
+        key = (id(ddim),) + (key or (direction, grad is not None))
         ent = cache.get(key)
         if ent is None:
             with torch.inference_mode(False):   # never inference tensors: the cache outlives the caller's autograd mode
@@ -72,35 +83,44 @@ class _StepRunner:
             return hf["eps"], False
         return None, False
 
+    def _fuse_desc(self, is_grad_head: bool):
+        """Descriptor of the update fused into the head's epilogue (include/pdae_b200.h: pdae_conv_tc2_set_head_fuse), or None
+        to run the standalone update instead."""
+        d = self.d
+        tab = d.alphas_cumprod_prev if self.direction == "sample" else d.alphas_cumprod_next
+        Ce = int(self.eps.tensor.shape[1])
+        flags = 1 | (self.C << 8) | (Ce << 16)
+        if is_grad_head:
+            flags |= 2 if self.grad is not None else 4
+        return [flags, self.eps.tensor.data_ptr(), self.x_in.tensor.data_ptr(), self.ent["t_loc"].data_ptr(),
+                d.sqrt_recip_alphas_cumprod.data_ptr(), d.sqrt_recip_alphas_cumprod_m1.data_ptr(),
+                d.sqrt_one_minus_alphas_cumprod.data_ptr(), tab.data_ptr()]
+
+    def _update(self):
+        """The standalone update, inside the step graph."""
+        x = self.x_in.tensor
+        self.d._update(x, self.ent["t_loc"], self.eps.tensor, self.grad.tensor if self.grad is not None else None,
+                       self.direction, out=x)
+
     def _launch_step(self):
-        d, L = self.d, _native.lib()
-        st = _stream(d.device)
-        rc = L.pdae_ddim_select_t(_ptr(self.ent["counter"]), self.delta, _ptr(d.timestep_map), int(d.timestep_map.shape[0]),
+        L = _native.lib()
+        st = _stream(self.d.device)
+        rc = L.pdae_ddim_select_t(_ptr(self.ent["counter"]), self.delta, _ptr(self.tmap), int(self.tmap.shape[0]),
                                   _ptr(self.ent["t_loc"]), _ptr(self.t_in.tensor), self.B, st)
         _native.check(rc, "pdae_ddim_select_t")
         self.plan._launch_all()
         if self.in_graph_update and not self.fused:
-            x = self.x_in.tensor
-            d._update(x, self.ent["t_loc"], self.eps.tensor, self.grad.tensor if self.grad is not None else None,
-                      self.direction, out=x)
+            self._update()
 
     def begin(self):
         self.plan.run_prologue()          # forced weight re-pack + step-invariant ops (label_emb(z), emb_z_layers)
-        # DDIM update fused into the last head conv's epilogue: point its device-side descriptor at this loop's tables
+        # update fused into the last head conv's epilogue: point its device-side descriptor at this loop's tables
         fuse, is_grad_head = self._fuse_target()
-        self.fused = fuse is not None and self.in_graph_update
+        desc = self._fuse_desc(is_grad_head) if fuse is not None and self.in_graph_update else None
+        self.fused = desc is not None
         self.fuse_buf = fuse if self.fused else None
         if self.fused:
-            d = self.d
-            tab = d.alphas_cumprod_prev if self.direction == "sample" else d.alphas_cumprod_next
-            Ce = int(self.eps.tensor.shape[1])
-            flags = 1 | (self.C << 8) | (Ce << 16)
-            if is_grad_head:
-                flags |= 2 if self.grad is not None else 4
-            desc = [flags, self.eps.tensor.data_ptr(), self.x_in.tensor.data_ptr(), self.ent["t_loc"].data_ptr(),
-                    d.sqrt_recip_alphas_cumprod.data_ptr(), d.sqrt_recip_alphas_cumprod_m1.data_ptr(),
-                    d.sqrt_one_minus_alphas_cumprod.data_ptr(), tab.data_ptr()]
-            fuse.tensor.copy_(torch.tensor(desc, dtype=torch.int64))
+            fuse.tensor.copy_(torch.tensor(desc + [0] * (FUSE_DESC_LEN - len(desc)), dtype=torch.int64))
         gkey = "graph_fused" if self.fused else "graph"
         if self.ent.get(gkey) is None:
             self.seek(1 if self.direction == "sample" else 0)
@@ -126,6 +146,76 @@ class _StepRunner:
             x = self.x_in.tensor
             e = self.eps.tensor[:, :self.C].contiguous()
             self.d._update(x, self.ent["t_loc"], e, self.grad.tensor if self.grad is not None else None, self.direction, out=x)
+
+
+class _DDPMRunner(_StepRunner):
+    """A DDPM ancestral loop (gaussian_diffusion.py:216-229 regular, :257-270 representation learning) on the step graph:
+    the counter runs T-1 .. 0 over the identity map (t_loc = t_net = i); the caller writes each step's N(0, 1) draw into
+    `noise` before `step()`.  The update is fused into the last tensor-core head (UNet epsilon head; ShiftUNet shift head,
+    eps + shift_coef[t] * grad) or runs as pdae_noise_p_sample_shift inside the graph (fp32 / CUDA-core heads, learned
+    sigma: epsilon and log-variance range are the two halves of the 2C output)."""
+
+    def __init__(self, gd, plan, x_in, t_in, eps, grad, C: int):
+        super().__init__(gd, plan, x_in, t_in, eps, grad, "ddpm", C, tmap=gd.identity_map(), key=("ddpm", grad is not None))
+        self.in_graph_update = True
+        if "noise" not in self.ent:
+            with torch.inference_mode(False):
+                self.ent["noise"] = torch.zeros_like(x_in.tensor)
+        self.noise = self.ent["noise"]
+        if eps.tensor.shape[1] != C and gd._log_betas is None:
+            gd._log_betas = torch.log(gd.betas)
+
+    def _fuse_desc(self, is_grad_head: bool):
+        gd, C = self.d, self.C
+        if self.eps.tensor.shape[1] != C:       # learned sigma: epsilon and range sit in different lanes of the head
+            return None
+        flags = 1 | 8 | (2 if self.grad is not None else 0) | (C << 8) | (C << 16)
+        return [flags, self.eps.tensor.data_ptr(), self.x_in.tensor.data_ptr(), self.ent["t_loc"].data_ptr(),
+                gd.noise_posterior_mean_x_t_coef.data_ptr(), gd.noise_posterior_mean_noise_coef.data_ptr(),
+                gd.shift_coef.data_ptr(), gd.posterior_log_variance_clipped.data_ptr(), self.noise.data_ptr()]
+
+    def _update(self):
+        gd, x, e = self.d, self.x_in.tensor, self.eps.tensor
+        per = x.numel() // self.B
+        lr = ctypes.c_void_p(e.data_ptr() + per * e.element_size()) if e.shape[1] != self.C else None
+        rc = _native.lib().pdae_noise_p_sample_shift(
+            _ptr(x), _ptr(e), _ptr(self.grad.tensor if self.grad is not None else None), _ptr(gd.shift_coef), _ptr(self.noise),
+            lr, e.numel() // self.B, _ptr(self.ent["t_loc"]), _ptr(gd.noise_posterior_mean_x_t_coef),
+            _ptr(gd.noise_posterior_mean_noise_coef), _ptr(gd.posterior_log_variance_clipped), _ptr(gd._log_betas), _ptr(x),
+            self.B, per, _stream(x.device))
+        _native.check(rc, "pdae_noise_p_sample_shift")
+
+
+class _InterpRunner(_StepRunner):
+    """DDIM trajectory interpolation (ddim.py:149-174) on ShiftUNet.plan_for_interp: epsilon and the frozen half once, the
+    shift half for z_1 and z_2; the update (gradient (1 - alpha) g1 + alpha g2, then the DDIM step) is fused into the second
+    shift head or runs as pdae_grad_blend + pdae_ddim_step inside the graph.  alpha lives in device memory (the descriptor,
+    `ab`), so one captured graph serves every alpha."""
+
+    def __init__(self, ddim, plan, x_in, t_in, eps, g1, g2, C: int, alpha):
+        super().__init__(ddim, plan, x_in, t_in, eps, g2, "sample", C, key=("interp",))
+        self.g1 = g1
+        if "ab" not in self.ent:
+            with torch.inference_mode(False):
+                self.ent["ab"] = torch.zeros(2, dtype=torch.float32, device=ddim.device)
+                self.ent["g"] = torch.zeros_like(g2.tensor)
+        self.ab = np.array([1.0 - alpha, alpha], dtype=np.float32)   # torch's fp32 scalars of (1.0 - alpha) * g1 + alpha * g2
+
+    def begin(self):
+        self.ent["ab"].copy_(torch.from_numpy(self.ab))
+        super().begin()
+
+    def _fuse_desc(self, is_grad_head: bool):
+        desc = super()._fuse_desc(is_grad_head)
+        desc[0] |= 16
+        return desc + [self.g1.tensor.data_ptr(), int(self.ab.view(np.int64)[0])]
+
+    def _update(self):
+        x, g = self.x_in.tensor, self.ent["g"]
+        rc = _native.lib().pdae_grad_blend(_ptr(self.g1.tensor), _ptr(self.grad.tensor), _ptr(self.ent["ab"]), _ptr(g),
+                                           g.numel(), _stream(x.device))
+        _native.check(rc, "pdae_grad_blend")
+        self.d._update(x, self.ent["t_loc"], self.eps.tensor, g, "sample", out=x)
 
 
 class DDIM:
@@ -187,11 +277,9 @@ class DDIM:
 
     def _loop(self, net, x, cond, direction, shift, stop_step=0):
         from ..model.shift_unet import ShiftUNet
-        from ..model.unet import UNet
         B = x.shape[0]
-        fast = isinstance(net, (ShiftUNet, UNet)) and x.is_cuda and x.dim() == 4 and not torch.is_grad_enabled()
         ts = torch.arange(0, self.timesteps + 1, device=self.device, dtype=torch.int64)
-        if not fast:
+        if not graphable(net, x):
             img = x
             for i in self._steps(direction):
                 t = ts[i].expand(B).contiguous()
@@ -217,7 +305,7 @@ class DDIM:
                 p2, (x2, t2, _, eps2, _) = net.plan_for(B, H, W, with_shift=False)
                 tail = _StepRunner(self, p2, x2, t2, eps2, None, direction, C)
         else:
-            plan, (x_in, t_in, c_in, eps) = net._get_plan(("unet", B, H, W), lambda P: net._build(P, B, H, W))
+            plan, (x_in, t_in, c_in, eps) = net.plan_for(B, H, W)
             if c_in is not None:
                 c_in.tensor.copy_(cond)
             main = _StepRunner(self, plan, x_in, t_in, eps, None, direction, C)
@@ -255,8 +343,27 @@ class DDIM:
         return self._loop(decoder, x_0, z, "encode", shift=True)
 
     def shift_ddim_trajectory_interpolation(self, decoder, z_1, z_2, x_T, alpha):
-        """ddim.py:149-174: two decoder calls per step, gradient = (1-alpha) g1 + alpha g2, epsilon from the first."""
+        """ddim.py:149-174: two decoder calls per step, gradient = (1-alpha) g1 + alpha g2, epsilon from the first.
+        On a ShiftUNet a step is one graph of the interpolation plan: the frozen half (and epsilon) is evaluated once, only
+        the shift half runs for both z (ShiftUNet.plan_for_interp)."""
+        from ..model.shift_unet import ShiftUNet
         B = x_T.shape[0]
+        if (isinstance(decoder, ShiftUNet) and graphable(decoder, x_T)
+                and decoder.output_channel == x_T.shape[1]):   # (learned sigma: the generic loop raises)
+            _, C, H, W = x_T.shape
+            plan, (x_in, t_in, z1_in, z2_in, eps, g1, g2) = decoder.plan_for_interp(B, H, W)
+            z1_in.tensor.copy_(z_1)
+            z2_in.tensor.copy_(z_2)
+            run = _InterpRunner(self, plan, x_in, t_in, eps, g1, g2, C, alpha)
+            run.begin()
+            try:
+                x_in.tensor.copy_(x_T)
+                run.seek(self.timesteps)
+                for _ in range(self.timesteps):
+                    run.step()
+                return x_in.tensor.clone()
+            finally:
+                run.end()
         x_t = x_T
         for i in reversed(range(1, self.timesteps + 1)):
             t = torch.full((B,), i, device=self.device, dtype=torch.long)

@@ -17,7 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _native
-from .ddim import DDIM, _f32, _ptr, _stream, _t64
+from .ddim import DDIM, _DDPMRunner, _f32, _ptr, _stream, _t64, graphable
 
 
 def _beta_schedule(kind: str, T: int) -> np.ndarray:
@@ -205,7 +205,44 @@ class GaussianDiffusion:
             return torch.split(output, C, dim=1)
         return output, None
 
+    def identity_map(self):
+        """arange(T) on the device: the timestep map of the DDPM loops' device-side step counter (t_loc = t_net = i)."""
+        m = self.__dict__.get("_identity_map")
+        if m is None:
+            with torch.inference_mode(False):
+                m = torch.arange(self.timesteps, dtype=torch.int64, device=self.device)
+            self.__dict__["_identity_map"] = m
+        return m
+
+    def _ddpm_graphed(self, net, x_T, cond, shift):
+        """A DDPM loop on the one-graph-per-step path (ddim._DDPMRunner): the network's static plan buffers are driven in
+        place; per step the host draws the noise exactly as the generic loop does (self._randn, once per step, same order),
+        copies it into the step's static noise buffer and replays the graph."""
+        B, C, H, W = x_T.shape
+        if shift:
+            plan, (x_in, t_in, z_in, eps, grad) = net.plan_for(B, H, W)
+            z_in.tensor.copy_(cond)
+        else:
+            plan, (x_in, t_in, c_in, eps) = net.plan_for(B, H, W)
+            grad = None
+            if c_in is not None:
+                c_in.tensor.copy_(cond)
+        run = _DDPMRunner(self, plan, x_in, t_in, eps, grad, C)
+        run.begin()
+        try:
+            x_in.tensor.copy_(x_T)
+            run.seek(self.timesteps - 1)
+            for _ in range(self.timesteps):
+                run.noise.copy_(self._randn(x_T.shape))
+                run.step()
+            return x_in.tensor.clone()
+        finally:
+            run.end()
+
     def regular_ddpm_sample(self, denoise_fn, x_T, condition=None):
+        from ..model.unet import UNet
+        if isinstance(denoise_fn, UNet) and graphable(denoise_fn, x_T):
+            return self._ddpm_graphed(denoise_fn, x_T, condition, shift=False)
         B, C = x_T.shape[0], x_T.shape[1]
         img = x_T
         for i in reversed(range(self.timesteps)):
@@ -228,6 +265,10 @@ class GaussianDiffusion:
         s = x_0.shape
         if z is None:
             z = encoder(x_0)
+        from ..model.shift_unet import ShiftUNet
+        if (isinstance(decoder, ShiftUNet) and graphable(decoder, x_T) and s[0] == x_T.shape[0]
+                and decoder.output_channel == x_T.shape[1]):   # (learned sigma: eps + coef * grad does not broadcast)
+            return self._ddpm_graphed(decoder, x_T, z, shift=True)
         img = x_T
         for i in reversed(range(self.timesteps)):
             t = torch.full((s[0],), i, device=self.device, dtype=torch.long)

@@ -28,6 +28,7 @@ from ._native import PDAE_BF16, PDAE_F32, RESAMPLE_DOWN2, RESAMPLE_NONE, RESAMPL
 
 _DT = {torch.float32: PDAE_F32, torch.bfloat16: PDAE_BF16}
 _STREAM = object()  # placeholder replaced by the current stream at run time
+FUSE_DESC_LEN = 10  # int64 slots of an image head's fused-update descriptor (include/pdae_b200.h: pdae_conv_tc2_set_head_fuse)
 
 _default_precision = "bf16"
 # "fp32"   : CUDA-core fp32 arithmetic everywhere (parity / training mode)
@@ -874,7 +875,7 @@ class Plan:
             fuse = None
             if fuse_key is not None:
                 with torch.inference_mode(False):
-                    fuse = self.fixed(torch.zeros(8, dtype=torch.int64, device=self.device))
+                    fuse = self.fixed(torch.zeros(FUSE_DESC_LEN, dtype=torch.int64, device=self.device))
                 self.head_fuse[fuse_key] = fuse
             self.call("conv_tc2", x, wp, self.param(bias), None, out_nchw, PDAE_F32, None, B, H, W, Ce, 16, 3, Cout, 0, fuse, flops=fl)
         elif Cout <= 4 and Cin % 4 == 0:

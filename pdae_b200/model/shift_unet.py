@@ -61,27 +61,31 @@ class ShiftUNet(PlannedModule):
             m.requires_grad_(requires_grad=False)
 
     # ---- plan ---------------------------------------------------------------------------------------
-    def _build(self, P: Plan, B: int, H: int, W: int, with_shift: bool = True):
+    def _build(self, P: Plan, B: int, H: int, W: int, with_shift: bool = True, interp: bool = False):
         """with_shift=False records only the frozen epsilon half (== the plain UNet): the plan a sampling loop replays on
-        its `use_shift=False` tail steps (ddim.py:119, stop_percent > 0), skipping ~45 % of the FLOPs."""
+        its `use_shift=False` tail steps (ddim.py:119, stop_percent > 0), skipping ~45 % of the FLOPs.
+        interp=True: the trajectory-interpolation plan (ddim.py:149-174) -- two z inputs, the frozen half and the epsilon
+        head once, one shift half per z on the same skip tensors; the second shift head is the plan's last op."""
         dev = self._device()
         E, base = self.time_embed_dim, self.base_channel
         x_in = P.new((B, self.input_channel, H, W), torch.float32, "x_nchw")
         t_in = P.new((B,), torch.int64, "t")
-        z_in = P.new((B, self.latent_dim), torch.float32, "z")
-        for b in (x_in, t_in, z_in):
+        z_ins = [P.new((B, self.latent_dim), torch.float32, n) for n in (("z", "z2") if interp else ("z",))]
+        for b in (x_in, t_in, *z_ins):
             b.keep = True
         shift_blocks = res_blocks_of(self.shift_middle_block, self.shift_output_blocks) if with_shift else []
-        bank_z = None
+        banks_z = []
         if with_shift:
             # z is constant over a sampling loop: label_emb(z) and every emb_z_layers Linear are step-invariant
             # (SURVEY.md §8(f) row 2) -- recorded as the plan's prologue, run once per loop instead of once per step
             with P.prologue():
-                shift_emb = P.new((B, E), torch.float32, "shift_emb")
-                shift_emb.keep = True
-                P.linear(z_in, self.label_emb.weight, self.label_emb.bias, shift_emb, B=B, Cin=self.latent_dim, Cout=E)
-                bank_z = EmbBank(P, shift_blocks, "z", shift_emb, B, E, "shift_z")
-                bank_z.out.keep = True
+                for z_in in z_ins:
+                    shift_emb = P.new((B, E), torch.float32, "shift_emb")
+                    shift_emb.keep = True
+                    P.linear(z_in, self.label_emb.weight, self.label_emb.bias, shift_emb, B=B, Cin=self.latent_dim, Cout=E)
+                    bank_z = EmbBank(P, shift_blocks, "z", shift_emb, B, E, "shift_z")
+                    bank_z.out.keep = True
+                    banks_z.append(bank_z)
         emb = emit_time_embed(P, self.time_embed, t_in, B, base, E, dev)
         bank_t = EmbBank(P, res_blocks_of(self.input_blocks, self.middle_block, self.output_blocks) + shift_blocks, "t",
                          emb, B, E, "shift_t" if with_shift else "eps_t")
@@ -92,27 +96,35 @@ class ShiftUNet(PlannedModule):
             h = stage.emit(P, h, bank_t)
             hs.append(h)
         eps_h = self.middle_block.emit(P, h, bank_t)
-        shift_h = self.shift_middle_block.emit(P, h, bank_t, bank_z) if with_shift else None
+        shift_hs = [self.shift_middle_block.emit(P, h, bank_t, bank_z) for bank_z in banks_z]
         for stage, shift_stage in zip(self.output_blocks, self.shift_output_blocks):
             skip = hs.pop()
             eps_h = stage.emit(P, eps_h.cat(skip), bank_t)
-            if with_shift:
-                shift_h = shift_stage.emit(P, shift_h.cat(skip), bank_t, bank_z)
+            shift_hs = [shift_stage.emit(P, sh.cat(skip), bank_t, bank_z) for sh, bank_z in zip(shift_hs, banks_z)]
         eps = P.new((B, self.output_channel, H, W), torch.float32, "eps_nchw")
         eps.keep = True
         emit_head(P, self.out, eps_h, eps, fuse_key=None if with_shift else "eps")
-        grad = None
-        if with_shift:
+        grads = []
+        for k, shift_h in enumerate(shift_hs):
             grad = P.new((B, self.input_channel, H, W), torch.float32, "shift_nchw")
             grad.keep = True
-            emit_head(P, self.shift_out, shift_h, grad, fuse_key="grad")   # the step's LAST op: may carry the fused DDIM update
-        return x_in, t_in, z_in, eps, grad
+            last = k == len(shift_hs) - 1   # the step's LAST op: may carry the fused sampling update
+            emit_head(P, self.shift_out, shift_h, grad, fuse_key="grad" if last else None)
+            grads.append(grad)
+        if interp:
+            return x_in, t_in, z_ins[0], z_ins[1], eps, grads[0], grads[1]
+        return x_in, t_in, z_ins[0], eps, grads[0] if grads else None
 
     def plan_for(self, B: int, H: int, W: int, with_shift: bool = True):
         """(plan, (x_in, t_in, z_in, eps, grad)) -- static buffers a sampling loop can drive directly.
         with_shift=False: the epsilon-only plan (grad is None, z_in unused)."""
         return self._get_plan(("shiftunet" if with_shift else "shiftunet_eps", B, H, W, self.training),
                               lambda P: self._build(P, B, H, W, with_shift))
+
+    def plan_for_interp(self, B: int, H: int, W: int):
+        """(plan, (x_in, t_in, z1_in, z2_in, eps, g1, g2)) -- the trajectory-interpolation plan (see _build)."""
+        return self._get_plan(("shiftunet_interp", B, H, W, self.training),
+                              lambda P: self._build(P, B, H, W, interp=True))
 
     def forward(self, x, time, condition):
         """x [N,3,H,W], time int64 [N], condition = z [N, latent_dim] -> (epsilon, shift), both NCHW fp32."""

@@ -202,6 +202,10 @@ class UNet(PlannedModule):
         emit_head(P, self.out, h, out, fuse_key="eps")
         return x_in, t_in, c_in, out
 
+    def plan_for(self, B: int, H: int, W: int):
+        """(plan, (x_in, t_in, c_in, eps)) -- static buffers a sampling loop can drive directly (c_in: class labels or None)."""
+        return self._get_plan(("unet", B, H, W), lambda P: self._build(P, B, H, W))
+
     def forward(self, x, time, condition=None):
         """x [N,C,H,W] fp32, time int64 [N], condition int64 [N] if class-conditional -> [N,C(|2C),H,W]."""
         if self.num_class is not None:
@@ -213,7 +217,7 @@ class UNet(PlannedModule):
             return unet_train_forward(self, x.contiguous(), time, condition)
         B, C, H, W = x.shape
         assert C == self.input_channel
-        plan, (x_in, t_in, c_in, out) = self._get_plan(("unet", B, H, W), lambda P: self._build(P, B, H, W))
+        plan, (x_in, t_in, c_in, out) = self.plan_for(B, H, W)
         x_in.tensor.copy_(x)
         t_in.tensor.copy_(time)
         if c_in is not None:
