@@ -155,6 +155,15 @@ int pdae_mlp_mod_ln_act_bf16(const float* h, const float* cond, int cond_ld, con
                              int silu, const float* mask, float mask_scale, void* out_bf16, int out_ld, int B, int N,
                              pdae_stream_t stream);
 int pdae_copy_cols_bf16(const float* src, void* dst_bf16, int dst_ld, int col0, int B, int N, pdae_stream_t stream);
+/* split operands of the latent MLP's sampling forward in the tensor-core modes.  out / dst: bf16 [B][3 * ld], the column
+ * blocks [hi | lo | hi] of a split-operand concat buffer (hi = bf16_rn(v), lo = bf16_rn(v - hi), as pdae_gn_apply_split3
+ * rounds them); columns col0 .. col0 + N - 1 of each block are written (col0 + N <= ld).
+ * pdae_mlp_mod_ln_act_split3: v = exactly what pdae_mlp_mod_ln_act computes in fp32, cond row b at cond + b * cond_ld;
+ * cond_ld = 0 reads one cond row for every row (a batch that shares its timestep).
+ * pdae_copy_cols_split3: v = src[b][j] (src row stride N).                                                            */
+int pdae_mlp_mod_ln_act_split3(const float* h, const float* cond, int cond_ld, const float* ln_w, const float* ln_b, float eps,
+                               int silu, void* out_split3, int ld, int col0, int B, int N, pdae_stream_t stream);
+int pdae_copy_cols_split3(const float* src, void* dst_split3, int ld, int col0, int B, int N, pdae_stream_t stream);
 
 
 /* ---- backward (training config: autograd through module.py:278-297,361-384,422-428 and the encoders), fp32 ---------

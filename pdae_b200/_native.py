@@ -77,6 +77,8 @@ _SIGS = {
     "pdae_copy_cols": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     "pdae_mlp_mod_ln_act_bf16": (c_int, [_P, _P, c_int, _P, _P, c_float, c_int, _P, c_float, _P, c_int, c_int, c_int, _P]),
     "pdae_copy_cols_bf16": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
+    "pdae_mlp_mod_ln_act_split3": (c_int, [_P, _P, c_int, _P, _P, c_float, c_int, _P, c_int, c_int, c_int, c_int, _P]),
+    "pdae_copy_cols_split3": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     "pdae_conv2d_dgrad_simt": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_conv2d_wgrad_simt": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_colsum": (c_int, [_P, c_int64, c_int, _P, _P]),

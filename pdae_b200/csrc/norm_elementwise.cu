@@ -577,15 +577,32 @@ __global__ void grad_blend_kernel(const float* __restrict__ g1, const float* __r
     out[i] = __fadd_rn(__fmul_rn(a1, g1[i]), __fmul_rn(a2, g2[i]));
 }
 
+// OutT of the latent MLP's row kernels in the split-operand plan: a value v is stored as hi = bf16_rn(v) at p, lo =
+// bf16_rn(v - hi) at p + blk and hi again at p + 2 blk -- the [hi | lo | hi] column blocks of a [B][3 blk] split operand,
+// rounded as store_split3 rounds them.
+struct Split3 {
+  __nv_bfloat16 v;
+};
+template <typename OutT>
+__device__ __forceinline__ void store_row(OutT* p, int, float v) { store1(p, v); }
+__device__ __forceinline__ void store_row(Split3* p, int blk, float v) {
+  __nv_bfloat16* q = reinterpret_cast<__nv_bfloat16*>(p);
+  const __nv_bfloat16 hi = __float2bfloat16_rn(v);
+  const __nv_bfloat16 lo = __float2bfloat16_rn(v - __bfloat162float(hi));
+  q[0] = hi;
+  q[blk] = lo;
+  q[2 * blk] = hi;
+}
+
 // one CTA per row: y = act(LN(h*(1+cond))) (* mask * scale, the inverted dropout of pdae_mul_mask_cols); cond row b at
 // cond + b * cond_ld.  OutT = float: pdae_mlp_mod_ln_act.  OutT = bf16: the next Linear's tensor-core operand, bf16_rn of
-// exactly the fp32 value (same reduction order, same expressions).
+// exactly the fp32 value (same reduction order, same expressions).  OutT = Split3: the split of that fp32 value (blk apart).
 template <typename OutT>
 __global__ void __launch_bounds__(256) mlp_mod_ln_act_kernel(const float* __restrict__ h, const float* __restrict__ cond,
                                                              int cond_ld, const float* __restrict__ lw,
                                                              const float* __restrict__ lb, float eps, int silu,
                                                              const float* __restrict__ mask, float scale,
-                                                             OutT* __restrict__ out, int out_ld, int N) {
+                                                             OutT* __restrict__ out, int out_ld, int N, int blk) {
   __shared__ float red[2][8];
   const int b = blockIdx.x;
   const float* hr = h + (long long)b * N;
@@ -620,17 +637,17 @@ __global__ void __launch_bounds__(256) mlp_mod_ln_act_kernel(const float* __rest
     if (lw) v = (v - mean) * rstd * lw[j] + lb[j];
     if (silu) v = silu_f(v);
     if (mask) v *= mask[(long long)b * N + j] * scale;
-    store1(out + (long long)b * out_ld + j, v);
+    store_row(out + (long long)b * out_ld + j, blk, v);
   }
 }
 
 template <typename OutT>
 __global__ void copy_cols_kernel(const float* __restrict__ src, OutT* __restrict__ dst, int dst_ld, int col0, int B,
-                                 int N) {
+                                 int N, int blk) {
   const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= (long long)B * N) return;
   const int b = (int)(i / N), j = (int)(i % N);
-  store1(dst + (long long)b * dst_ld + col0 + j, src[i]);
+  store_row(dst + (long long)b * dst_ld + col0 + j, blk, src[i]);
 }
 
 }  // namespace pdae
@@ -914,7 +931,7 @@ extern "C" int pdae_mlp_mod_ln_act(const float* h, const float* cond, const floa
   PDAE_REQUIRE(h && out && B > 0 && N > 0 && out_ld >= N, "mlp_mod_ln_act: bad args");
   PDAE_REQUIRE(!ln_w || ln_b, "mlp_mod_ln_act: LayerNorm weight without bias");
   mlp_mod_ln_act_kernel<float><<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, N, ln_w, ln_b, eps, silu, nullptr, 1.0f, out,
-                                                                    out_ld, N);
+                                                                    out_ld, N, 0);
   PDAE_LAUNCH_CHECK("mlp_mod_ln_act_kernel");
   return PDAE_OK;
 }
@@ -925,14 +942,26 @@ extern "C" int pdae_mlp_mod_ln_act_bf16(const float* h, const float* cond, int c
   PDAE_REQUIRE(h && out_bf16 && B > 0 && N > 0 && out_ld >= N && (!cond || cond_ld >= N), "mlp_mod_ln_act_bf16: bad args");
   PDAE_REQUIRE(!ln_w || ln_b, "mlp_mod_ln_act_bf16: LayerNorm weight without bias");
   mlp_mod_ln_act_kernel<__nv_bfloat16><<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, cond_ld, ln_w, ln_b, eps, silu, mask,
-                                                                            mask_scale, (__nv_bfloat16*)out_bf16, out_ld, N);
+                                                                            mask_scale, (__nv_bfloat16*)out_bf16, out_ld, N, 0);
   PDAE_LAUNCH_CHECK("mlp_mod_ln_act_kernel<bf16>");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_mlp_mod_ln_act_split3(const float* h, const float* cond, int cond_ld, const float* ln_w, const float* ln_b,
+                                          float eps, int silu, void* out_split3, int ld, int col0, int B, int N,
+                                          pdae_stream_t stream) {
+  PDAE_REQUIRE(h && out_split3 && B > 0 && N > 0 && col0 >= 0 && col0 + N <= ld && (!cond || cond_ld == 0 || cond_ld >= N),
+               "mlp_mod_ln_act_split3: bad args (B=%d N=%d ld=%d col0=%d cond_ld=%d)", B, N, ld, col0, cond_ld);
+  PDAE_REQUIRE(!ln_w || ln_b, "mlp_mod_ln_act_split3: LayerNorm weight without bias");
+  mlp_mod_ln_act_kernel<Split3><<<B, 256, 0, (cudaStream_t)stream>>>(h, cond, cond_ld, ln_w, ln_b, eps, silu, nullptr, 1.0f,
+                                                                     (Split3*)out_split3 + col0, 3 * ld, N, ld);
+  PDAE_LAUNCH_CHECK("mlp_mod_ln_act_kernel<split3>");
   return PDAE_OK;
 }
 
 extern "C" int pdae_copy_cols(const float* src, float* dst, int dst_ld, int col0, int B, int N, pdae_stream_t stream) {
   PDAE_REQUIRE(src && dst && col0 >= 0 && col0 + N <= dst_ld, "copy_cols: bad args");
-  copy_cols_kernel<float><<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(src, dst, dst_ld, col0, B, N);
+  copy_cols_kernel<float><<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(src, dst, dst_ld, col0, B, N, 0);
   PDAE_LAUNCH_CHECK("copy_cols_kernel");
   return PDAE_OK;
 }
@@ -940,7 +969,16 @@ extern "C" int pdae_copy_cols(const float* src, float* dst, int dst_ld, int col0
 extern "C" int pdae_copy_cols_bf16(const float* src, void* dst_bf16, int dst_ld, int col0, int B, int N, pdae_stream_t stream) {
   PDAE_REQUIRE(src && dst_bf16 && B > 0 && N > 0 && col0 >= 0 && col0 + N <= dst_ld, "copy_cols_bf16: bad args");
   copy_cols_kernel<__nv_bfloat16><<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(
-      src, (__nv_bfloat16*)dst_bf16, dst_ld, col0, B, N);
+      src, (__nv_bfloat16*)dst_bf16, dst_ld, col0, B, N, 0);
   PDAE_LAUNCH_CHECK("copy_cols_kernel<bf16>");
+  return PDAE_OK;
+}
+
+extern "C" int pdae_copy_cols_split3(const float* src, void* dst_split3, int ld, int col0, int B, int N, pdae_stream_t stream) {
+  PDAE_REQUIRE(src && dst_split3 && B > 0 && N > 0 && col0 >= 0 && col0 + N <= ld,
+               "copy_cols_split3: bad args (B=%d N=%d ld=%d col0=%d)", B, N, ld, col0);
+  copy_cols_kernel<Split3><<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(src, (Split3*)dst_split3, 3 * ld,
+                                                                                         col0, B, N, ld);
+  PDAE_LAUNCH_CHECK("copy_cols_kernel<split3>");
   return PDAE_OK;
 }

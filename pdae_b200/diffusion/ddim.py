@@ -39,11 +39,14 @@ def _t64(t, B, what):
 
 
 def graphable(net, x) -> bool:
-    """Does a sampling loop over `net` run on the one-graph-per-step path (a pdae_b200 UNet / ShiftUNet on a 4-D CUDA input
-    with autograd off)?  Any other callable takes the generic per-step loop."""
+    """Does a sampling loop over `net` run on the one-graph-per-step path (a pdae_b200 UNet / ShiftUNet on a 4-D CUDA input,
+    or a pdae_b200 MLPSkipNet on a 2-D one, with autograd off)?  Any other callable takes the generic per-step loop."""
+    from ..model.mlp_skip_net import MLPSkipNet
     from ..model.shift_unet import ShiftUNet
     from ..model.unet import UNet
-    return isinstance(net, (ShiftUNet, UNet)) and x.is_cuda and x.dim() == 4 and not torch.is_grad_enabled()
+    if not x.is_cuda or torch.is_grad_enabled():
+        return False
+    return (isinstance(net, (ShiftUNet, UNet)) and x.dim() == 4) or (isinstance(net, MLPSkipNet) and x.dim() == 2)
 
 
 class _StepRunner:
@@ -279,7 +282,7 @@ class DDIM:
         from ..model.shift_unet import ShiftUNet
         B = x.shape[0]
         ts = torch.arange(0, self.timesteps + 1, device=self.device, dtype=torch.int64)
-        if not graphable(net, x):
+        if not graphable(net, x) or x.dim() != 4:   # (an MLPSkipNet's graphed loop is latent_ddim_sample_loop)
             img = x
             for i in self._steps(direction):
                 t = ts[i].expand(B).contiguous()
@@ -383,8 +386,23 @@ class DDIM:
         return z0 * torch.sqrt(ap) + torch.sqrt(1.0 - ap) * eps
 
     def latent_ddim_sample_loop(self, latent_denoise_fn, z_T):
-        """ddim.py:200-207 -- NB calls ddim_sample, i.e. WITH the clamp of the predicted z_0."""
+        """ddim.py:200-207 -- NB calls ddim_sample, i.e. WITH the clamp of the predicted z_0.
+        On a pdae_b200 MLPSkipNet a step is one graph: the timestep lookup, the network's plan for a batch that shares its
+        timestep (MLPSkipNet.plan_for(B, one_t=True)) and the clamped update written back into the plan's z_t input."""
+        from ..model.mlp_skip_net import MLPSkipNet
         B = z_T.shape[0]
+        if isinstance(latent_denoise_fn, MLPSkipNet) and graphable(latent_denoise_fn, z_T):
+            plan, (x_in, t_in, eps) = latent_denoise_fn.plan_for(B, one_t=True)
+            run = _StepRunner(self, plan, x_in, t_in, eps, None, "sample", z_T.shape[1], key=("latent",))
+            run.begin()
+            try:
+                x_in.tensor.copy_(z_T)
+                run.seek(self.timesteps)
+                for _ in range(self.timesteps):
+                    run.step()
+                return x_in.tensor.clone()
+            finally:
+                run.end()
         z = z_T
         for i in reversed(range(1, self.timesteps + 1)):
             t = torch.full((B,), i, device=self.device, dtype=torch.long)
