@@ -140,6 +140,17 @@ int pdae_noise_p_sample_shift(const float* x, const float* eps, const float* gra
 /* ddim.py:168 trajectory-interpolation gradient: out = ab[0]*g1 + ab[1]*g2 (fp32, one rounding per product and sum), with
  * ab = { fp32(1 - alpha), fp32(alpha) } in DEVICE memory.  out may alias g1 or g2.                      */
 int pdae_grad_blend(const float* g1, const float* g2, const float* ab, float* out, int64_t n, pdae_stream_t stream);
+/* gaussian_diffusion.py:292-318 gap measure, one timestep: per element (fp32, one rounding per product and sum, tables indexed
+ * by t[b]) true = c0*x0 + c1*x_t; m1 = c0*(A*x_t - Bm*eps) + c1*x_t; m2 = the same with eps + shift*grad; then
+ * out[2*t[0]] = mean((true - m1)^2), out[2*t[0] + 1] = mean((true - m2)^2) over all B*per_sample elements (the loop's t is
+ * shared by the batch, so t[0] picks the row on the device).  Tables: x_0_posterior_mean_x_0_coef, _x_t_coef,
+ * sqrt_recip_alphas_cumprod, _m1, shift_coef.  Deterministic: fp64 block partials over a grid fixed by the element count, summed
+ * in a fixed order, no atomics.  workspace: caller-owned device memory of pdae_gap_terms_workspace_bytes(B*per_sample) bytes
+ * (a negative result: total <= 0).                                                                                    */
+int64_t pdae_gap_terms_workspace_bytes(int64_t total);
+int pdae_gap_terms(const float* x0, const float* x_t, const float* eps, const float* grad, const int64_t* t, const float* tab_c0,
+                   const float* tab_c1, const float* tab_A, const float* tab_Bm, const float* tab_shift, double* workspace,
+                   int64_t workspace_bytes, float* out, int B, int64_t per_sample, pdae_stream_t stream);
 
 /* ---- latent MLP row op (mlp_skip_net.py:123-141) -------------------------------------------------
  * y = act( LN( h * (1 + cond) ) ) per row; cond/ln_w optional; act = SiLU if silu.  out has row stride

@@ -73,6 +73,8 @@ _SIGS = {
     "pdae_noise_p_sample": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int, c_int64, _P]),
     "pdae_noise_p_sample_shift": (c_int, [_P, _P, _P, _P, _P, _P, c_int64, _P, _P, _P, _P, _P, _P, c_int, c_int64, _P]),
     "pdae_grad_blend": (c_int, [_P, _P, _P, _P, c_int64, _P]),
+    "pdae_gap_terms_workspace_bytes": (c_int64, [c_int64]),
+    "pdae_gap_terms": (c_int, [_P, _P, _P, _P, _P, _P, _P, _P, _P, _P, _P, c_int64, _P, c_int, c_int64, _P]),
     "pdae_mlp_mod_ln_act": (c_int, [_P, _P, _P, _P, c_float, c_int, _P, c_int, c_int, c_int, _P]),
     "pdae_copy_cols": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     "pdae_mlp_mod_ln_act_bf16": (c_int, [_P, _P, c_int, _P, _P, c_float, c_int, _P, c_float, _P, c_int, c_int, c_int, _P]),

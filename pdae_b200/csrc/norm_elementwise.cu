@@ -577,6 +577,78 @@ __global__ void grad_blend_kernel(const float* __restrict__ g1, const float* __r
     out[i] = __fadd_rn(__fmul_rn(a1, g1[i]), __fmul_rn(a2, g2[i]));
 }
 
+// The gap measure's per-step terms (gaussian_diffusion.py:292-318) in fp32, in the reference's expression order (one rounding
+// per product and per sum): true = c0 x0 + c1 xt; m1 = c0 (A xt - Bm eps) + c1 xt; m2 the same with eps + S grad; then
+// (true - m1)^2 and (true - m2)^2.  Each block sums GAP_PER_BLOCK consecutive elements in fp64 in a fixed order and writes its
+// two partials; the grid follows the element count only, so the partials -- and the final sum -- are the same on every run.
+constexpr int GAP_THREADS = 256;
+constexpr int GAP_ITEMS = 16;
+constexpr long long GAP_PER_BLOCK = (long long)GAP_THREADS * GAP_ITEMS;
+
+__device__ __forceinline__ void gap_block_sum(double& a, double& b, double (*red)[GAP_THREADS / 32]) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    a += __shfl_xor_sync(0xffffffffu, a, o);
+    b += __shfl_xor_sync(0xffffffffu, b, o);
+  }
+  if ((threadIdx.x & 31) == 0) { red[0][threadIdx.x >> 5] = a; red[1][threadIdx.x >> 5] = b; }
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    a = 0.0; b = 0.0;
+    for (int w = 0; w < GAP_THREADS / 32; ++w) { a += red[0][w]; b += red[1][w]; }
+  }
+}
+
+__global__ void __launch_bounds__(GAP_THREADS) gap_terms_partial_kernel(
+    const float* __restrict__ x0, const float* __restrict__ xt, const float* __restrict__ eps, const float* __restrict__ grad,
+    const int64_t* __restrict__ t, const float* __restrict__ c0, const float* __restrict__ c1, const float* __restrict__ tA,
+    const float* __restrict__ tBm, const float* __restrict__ tS, double* __restrict__ partial, long long per_sample,
+    long long total) {
+  __shared__ double red[2][GAP_THREADS / 32];
+  double s1 = 0.0, s2 = 0.0;
+  const long long base = (long long)blockIdx.x * GAP_PER_BLOCK + threadIdx.x;
+#pragma unroll 4
+  for (int k = 0; k < GAP_ITEMS; ++k) {
+    const long long i = base + (long long)k * GAP_THREADS;
+    if (i < total) {
+      const int64_t tb = t[i / per_sample];
+      const float a0 = c0[tb], a1 = c1[tb], A = tA[tb], Bm = tBm[tb];
+      const float x = xt[i], e = eps[i];
+      const float cx = __fmul_rn(a1, x), ax = __fmul_rn(A, x);
+      const float tru = __fadd_rn(__fmul_rn(a0, x0[i]), cx);
+      const float m1 = __fadd_rn(__fmul_rn(a0, __fsub_rn(ax, __fmul_rn(Bm, e))), cx);
+      const float eae = __fadd_rn(e, __fmul_rn(tS[tb], grad[i]));
+      const float m2 = __fadd_rn(__fmul_rn(a0, __fsub_rn(ax, __fmul_rn(Bm, eae))), cx);
+      const float d1 = __fsub_rn(tru, m1), d2 = __fsub_rn(tru, m2);
+      s1 += (double)__fmul_rn(d1, d1);
+      s2 += (double)__fmul_rn(d2, d2);
+    }
+  }
+  gap_block_sum(s1, s2, red);
+  if (threadIdx.x == 0) {
+    partial[2 * blockIdx.x] = s1;
+    partial[2 * blockIdx.x + 1] = s2;
+  }
+}
+
+// One block: the partials in a fixed order, then the two means into row t[0] of out ([T][2]).
+__global__ void __launch_bounds__(GAP_THREADS) gap_terms_final_kernel(const double* __restrict__ partial, int nblk,
+                                                                      const int64_t* __restrict__ t, float* __restrict__ out,
+                                                                      double total) {
+  __shared__ double red[2][GAP_THREADS / 32];
+  double s1 = 0.0, s2 = 0.0;
+  for (int j = threadIdx.x; j < nblk; j += GAP_THREADS) {
+    s1 += partial[2 * j];
+    s2 += partial[2 * j + 1];
+  }
+  gap_block_sum(s1, s2, red);
+  if (threadIdx.x == 0) {
+    float* row = out + 2 * t[0];
+    row[0] = (float)(s1 / total);
+    row[1] = (float)(s2 / total);
+  }
+}
+
 // OutT of the latent MLP's row kernels in the split-operand plan: a value v is stored as hi = bf16_rn(v) at p, lo =
 // bf16_rn(v - hi) at p + blk and hi again at p + 2 blk -- the [hi | lo | hi] column blocks of a [B][3 blk] split operand,
 // rounded as store_split3 rounds them.
@@ -923,6 +995,38 @@ extern "C" int pdae_grad_blend(const float* g1, const float* g2, const float* ab
   PDAE_REQUIRE(g1 && g2 && ab && out && n > 0, "grad_blend: bad args");
   grad_blend_kernel<<<ew_grid(n), 256, 0, (cudaStream_t)stream>>>(g1, g2, ab, out, n);
   PDAE_LAUNCH_CHECK("grad_blend_kernel");
+  return PDAE_OK;
+}
+
+static inline long long gap_blocks(long long total) { return (total + GAP_PER_BLOCK - 1) / GAP_PER_BLOCK; }
+
+extern "C" int64_t pdae_gap_terms_workspace_bytes(int64_t total) {
+  if (total <= 0) {
+    ::pdae::set_error("gap_terms_workspace_bytes: total=%lld must be > 0", (long long)total);
+    return PDAE_EINVAL;
+  }
+  return gap_blocks(total) * 2 * (int64_t)sizeof(double);
+}
+
+extern "C" int pdae_gap_terms(const float* x0, const float* x_t, const float* eps, const float* grad, const int64_t* t,
+                              const float* tab_c0, const float* tab_c1, const float* tab_A, const float* tab_Bm,
+                              const float* tab_shift, double* workspace, int64_t workspace_bytes, float* out, int B,
+                              int64_t per_sample, pdae_stream_t stream) {
+  PDAE_REQUIRE(x0 && x_t && eps && grad && t && tab_c0 && tab_c1 && tab_A && tab_Bm && tab_shift && workspace && out,
+               "gap_terms: null pointer");
+  PDAE_REQUIRE(B > 0 && per_sample > 0, "gap_terms: B=%d and per_sample=%lld must be > 0", B, (long long)per_sample);
+  const long long total = (long long)B * per_sample;
+  const long long nblk = gap_blocks(total);
+  PDAE_REQUIRE(nblk <= 0x7fffffffLL, "gap_terms: %lld elements are too many", total);
+  PDAE_REQUIRE(workspace_bytes >= nblk * 2 * (long long)sizeof(double),
+               "gap_terms: workspace of %lld bytes, %lld needed (pdae_gap_terms_workspace_bytes)", (long long)workspace_bytes,
+               nblk * 2 * (long long)sizeof(double));
+  cudaStream_t s = (cudaStream_t)stream;
+  gap_terms_partial_kernel<<<(unsigned)nblk, GAP_THREADS, 0, s>>>(x0, x_t, eps, grad, t, tab_c0, tab_c1, tab_A, tab_Bm,
+                                                                  tab_shift, workspace, per_sample, total);
+  PDAE_LAUNCH_CHECK("gap_terms_partial_kernel");
+  gap_terms_final_kernel<<<1, GAP_THREADS, 0, s>>>(workspace, (int)nblk, t, out, (double)total);
+  PDAE_LAUNCH_CHECK("gap_terms_final_kernel");
   return PDAE_OK;
 }
 

@@ -105,12 +105,13 @@ class _StepRunner:
         self.d._update(x, self.ent["t_loc"], self.eps.tensor, self.grad.tensor if self.grad is not None else None,
                        self.direction, out=x)
 
-    def _launch_step(self):
-        L = _native.lib()
-        st = _stream(self.d.device)
-        rc = L.pdae_ddim_select_t(_ptr(self.ent["counter"]), self.delta, _ptr(self.tmap), int(self.tmap.shape[0]),
-                                  _ptr(self.ent["t_loc"]), _ptr(self.t_in.tensor), self.B, st)
+    def _select_t(self):
+        rc = _native.lib().pdae_ddim_select_t(_ptr(self.ent["counter"]), self.delta, _ptr(self.tmap), int(self.tmap.shape[0]),
+                                              _ptr(self.ent["t_loc"]), _ptr(self.t_in.tensor), self.B, _stream(self.d.device))
         _native.check(rc, "pdae_ddim_select_t")
+
+    def _launch_step(self):
+        self._select_t()
         self.plan._launch_all()
         if self.in_graph_update and not self.fused:
             self._update()
@@ -187,6 +188,48 @@ class _DDPMRunner(_StepRunner):
             _ptr(gd.noise_posterior_mean_noise_coef), _ptr(gd.posterior_log_variance_clipped), _ptr(gd._log_betas), _ptr(x),
             self.B, per, _stream(x.device))
         _native.check(rc, "pdae_noise_p_sample_shift")
+
+
+class _GapRunner(_StepRunner):
+    """The gap measure (gaussian_diffusion.py:292-318) on the step graph of a ShiftUNet plan: the counter runs T-1 .. 0 over
+    the identity map; a step is pdae_q_sample of the static x_0 and noise buffers into the plan's input, the network, and
+    pdae_gap_terms writing both mean squared gaps into row t of the static [T][2] buffer `gaps`.  The caller writes x_0 once
+    and each step's uniform draw into `noise` before `step()`.  Nothing is fused into the heads: a plain forward afterwards
+    sees the plan unchanged."""
+
+    def __init__(self, gd, plan, x_in, t_in, eps, grad, C: int):
+        super().__init__(gd, plan, x_in, t_in, eps, grad, "gap", C, tmap=gd.identity_map(), key=("gap",))
+        self.in_graph_update = True
+        if "gaps" not in self.ent:
+            ws = _native.lib().pdae_gap_terms_workspace_bytes(x_in.tensor.numel())
+            if ws < 0:
+                _native.check(ws, "pdae_gap_terms_workspace_bytes")
+            with torch.inference_mode(False):
+                self.ent["x0"] = torch.zeros_like(x_in.tensor)
+                self.ent["noise"] = torch.zeros_like(x_in.tensor)
+                self.ent["gaps"] = torch.zeros(gd.timesteps, 2, dtype=torch.float32, device=gd.device)
+                self.ent["ws"] = torch.empty(ws // 8, dtype=torch.float64, device=gd.device)
+        self.x0, self.noise, self.gaps, self.ws = self.ent["x0"], self.ent["noise"], self.ent["gaps"], self.ent["ws"]
+
+    def _fuse_desc(self, is_grad_head: bool):
+        return None
+
+    def _launch_step(self):
+        L, gd = _native.lib(), self.d
+        st = _stream(gd.device)
+        t = self.ent["t_loc"]
+        self._select_t()
+        x = self.x_in.tensor
+        per = x.numel() // self.B
+        rc = L.pdae_q_sample(_ptr(self.x0), _ptr(self.noise), _ptr(t), _ptr(gd.sqrt_alphas_cumprod),
+                             _ptr(gd.sqrt_one_minus_alphas_cumprod), _ptr(x), self.B, per, st)
+        _native.check(rc, "pdae_q_sample")
+        self.plan._launch_all()
+        rc = L.pdae_gap_terms(_ptr(self.x0), _ptr(x), _ptr(self.eps.tensor), _ptr(self.grad.tensor), _ptr(t),
+                              _ptr(gd.x_0_posterior_mean_x_0_coef), _ptr(gd.x_0_posterior_mean_x_t_coef),
+                              _ptr(gd.sqrt_recip_alphas_cumprod), _ptr(gd.sqrt_recip_alphas_cumprod_m1), _ptr(gd.shift_coef),
+                              _ptr(self.ws), self.ws.numel() * 8, _ptr(self.gaps), self.B, per, st)
+        _native.check(rc, "pdae_gap_terms")
 
 
 class _InterpRunner(_StepRunner):

@@ -17,7 +17,7 @@ import torch
 import torch.nn.functional as F
 
 from .. import _native
-from .ddim import DDIM, _DDPMRunner, _f32, _ptr, _stream, _t64, graphable
+from .ddim import DDIM, _DDPMRunner, _GapRunner, _f32, _ptr, _stream, _t64, graphable
 
 
 def _beta_schedule(kind: str, T: int) -> np.ndarray:
@@ -291,10 +291,35 @@ class GaussianDiffusion:
         x_T = self.representation_learning_ddim_encode(encoder_ddim_style, encoder, decoder, x_0, z)
         return self.representation_learning_ddim_sample(decoder_ddim_style, None, decoder, None, x_T, z)
 
+    def _gap_graphed(self, decoder, x_0, z):
+        """The gap measure on the one-graph-per-step path (ddim._GapRunner): x_0 and z are written once into static buffers;
+        per step the host draws the uniform noise exactly as the generic loop does (self._rand_like, once per step, same
+        order), copies it into the step's static noise buffer and replays the graph.  The [T][2] results reach the host once."""
+        B, C, H, W = x_0.shape
+        plan, (x_in, t_in, z_in, eps, grad) = decoder.plan_for(B, H, W)
+        z_in.tensor.copy_(z)
+        run = _GapRunner(self, plan, x_in, t_in, eps, grad, C)
+        run.x0.copy_(_f32(x_0))
+        run.begin()
+        try:
+            run.seek(self.timesteps - 1)
+            for _ in range(self.timesteps):
+                run.noise.copy_(self._rand_like(x_0))
+                run.step()
+            gaps = run.gaps.cpu().flip(0)          # row t -> the reference's order t = T-1 .. 0
+        finally:
+            run.end()
+        return gaps[:, 0].tolist(), gaps[:, 1].tolist()
+
     def representation_learning_gap_measure(self, encoder, decoder, x_0):
-        """(:292-318) -- NB the reference draws its 'noise' with torch.rand_like (uniform); kept."""
+        """(:292-318) -- NB the reference draws its 'noise' with torch.rand_like (uniform); kept.
+        On a pdae_b200 ShiftUNet (grad off, epsilon-only output) a step is one CUDA graph and the gaps are reduced on the
+        device (_gap_graphed); any other decoder takes the generic loop below."""
         s = x_0.shape
         z = encoder(x_0)
+        from ..model.shift_unet import ShiftUNet
+        if isinstance(decoder, ShiftUNet) and graphable(decoder, x_0) and decoder.output_channel == s[1]:
+            return self._gap_graphed(decoder, x_0, z)
         gap_pred, gap_ae = [], []
         for i in reversed(range(self.timesteps)):
             t = torch.full((s[0],), i, device=self.device, dtype=torch.long)
