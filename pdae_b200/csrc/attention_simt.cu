@@ -284,11 +284,11 @@ extern "C" int pdae_qkv_split3(const float* qkv, void* Q3, void* K3, void* VT3, 
   const long long hs = legacy ? 3LL * ch : ch, ko = legacy ? ch : C, vo = legacy ? 2LL * ch : 2LL * C;
   PDAE_REQUIRE((long long)B * heads <= 65535, "qkv_split3: B*heads too large");
   PDAE_REQUIRE(ch % 8 == 0 && C % 4 == 0, "qkv_split3: C/heads=%d must be a multiple of 8", ch);
+  PDAE_REQUIRE(T % 2 == 0, "qkv_split3: T must be even");
   const long long total = (long long)B * heads * T * (ch / 8);
   cudaStream_t s = (cudaStream_t)stream;
   qk_split3_kernel<<<cdiv(total, 256), 256, 0, s>>>(qkv, (__nv_bfloat16*)Q3, (__nv_bfloat16*)K3, T, 3 * C, ch, heads, ko, hs, total);
   PDAE_LAUNCH_CHECK("qk_split3_kernel");
-  PDAE_REQUIRE(T % 2 == 0, "qkv_split3: T must be even");
   dim3 grid(cdiv(T, 64), cdiv(ch, 32), B * heads);
   v_split3_transpose_kernel<<<grid, 256, 0, s>>>(qkv, (__nv_bfloat16*)VT3, T, 3 * C, ch, heads, vo, hs);
   PDAE_LAUNCH_CHECK("v_split3_transpose_kernel");

@@ -718,6 +718,8 @@ extern "C" int pdae_gn_bwd_sums(const float* src1, int C1, const float* src2, in
   if (!src2) C2 = 0;
   const int C = C1 + C2;
   PDAE_REQUIRE(C1 % 4 == 0 && C2 % 4 == 0 && C % 32 == 0 && (size_t)2 * C * 4 <= 48 * 1024, "gn_bwd_sums: bad channels");
+  PDAE_REQUIRE(resample >= 0 && resample <= 2, "gn_bwd_sums: bad resample mode");
+  PDAE_REQUIRE(resample != PDAE_RESAMPLE_DOWN2 || (H % 2 == 0 && W % 2 == 0), "gn_bwd_sums: odd dims for DOWN2");
   cudaStream_t s = (cudaStream_t)stream;
   PDAE_CUDA(cudaMemsetAsync(S, 0, (size_t)B * C * 2 * sizeof(float), s));
   int ppc = 256;                                   // low-resolution layers: fewer pixels per CTA so that >= ~4 CTAs/SM exist
@@ -748,6 +750,8 @@ extern "C" int pdae_gn_bwd_apply(const float* src1, int C1, const float* src2, i
   PDAE_REQUIRE(src1 && ab && kk && dy && dx1, "gn_bwd_apply: null pointer");
   if (!src2) C2 = 0;
   PDAE_REQUIRE(C1 % 4 == 0 && C2 % 4 == 0 && !(dx2 && !src2), "gn_bwd_apply: bad channels");
+  PDAE_REQUIRE(resample >= 0 && resample <= 2, "gn_bwd_apply: bad resample mode");
+  PDAE_REQUIRE(resample != PDAE_RESAMPLE_DOWN2 || (H % 2 == 0 && W % 2 == 0), "gn_bwd_apply: odd dims for DOWN2");
   const long long items = (long long)H * W * ((dx2 ? C1 + C2 : C1) / 4);
   int gx = cdiv(items, 256);
   if (gx > 148 * 16) gx = 148 * 16;

@@ -833,6 +833,9 @@ extern "C" int pdae_gn_apply(const void* src1, int src1_dtype, int C1, const voi
   PDAE_REQUIRE(resample >= 0 && resample <= 2, "gn_apply: bad resample mode");
   PDAE_REQUIRE(resample != PDAE_RESAMPLE_DOWN2 || (H % 2 == 0 && W % 2 == 0), "gn_apply: odd dims for DOWN2");
   if (!out_raw) raw_dtype = (act_dtype == PDAE_BF16 && src1_dtype == PDAE_BF16 && src2_dtype == PDAE_BF16) ? PDAE_BF16 : PDAE_F32;
+  // each dtype is one bit of the dispatch key: any other value would alias a different combination
+  PDAE_REQUIRE(((unsigned)src1_dtype | (unsigned)src2_dtype | (unsigned)act_dtype | (unsigned)raw_dtype) <= 1u,
+               "gn_apply: unsupported dtype combination src1=%d src2=%d act=%d raw=%d", src1_dtype, src2_dtype, act_dtype, raw_dtype);
   cudaStream_t s = (cudaStream_t)stream;
   typedef __nv_bfloat16 bf;
   const int key = src1_dtype | (src2_dtype << 1) | (act_dtype << 2) | (raw_dtype << 3);

@@ -46,3 +46,22 @@ def test_sass_is_hopper_native():
     for mnem in ("HGMMA", "UTMALDG", "UTMASTG"):
         assert mnem in sass, mnem
     assert "sm_90a" in sass
+
+
+def test_gn_bwd_down2_rejects_odd_dims_before_any_launch():
+    """DOWN2 backward reads dy at (y/2, x/2) of an [H/2][W/2] tensor: an odd H or W would read past its end.  Both passes
+    that gather dy refuse it, like the forward, before touching the stream (dummy pointers are never dereferenced)."""
+    L = _native.lib()
+    p = ctypes.c_void_p(16)
+    for H, W in ((7, 8), (8, 9)):
+        rc = L.pdae_gn_bwd_sums(p, 64, None, 0, p, p, 1, 2, 2, H, W, p, None)
+        assert rc == -1 and b"odd dims for DOWN2" in L.pdae_last_error(), (H, W)
+        rc = L.pdae_gn_bwd_apply(p, 64, None, 0, p, p, p, 1, 2, 2, H, W, None, 0, p, None, None)
+        assert rc == -1 and b"odd dims for DOWN2" in L.pdae_last_error(), (H, W)
+
+
+def test_qkv_split3_rejects_odd_T_before_any_launch():
+    L = _native.lib()
+    p = ctypes.c_void_p(16)
+    rc = L.pdae_qkv_split3(p, p, p, p, 2, 63, 64, 2, 0, None)
+    assert rc == -1 and b"T must be even" in L.pdae_last_error()
