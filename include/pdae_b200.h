@@ -94,6 +94,16 @@ int pdae_ch_stats(const float* src, int B, int HW, int C, float* chs, pdae_strea
 int pdae_gn_coef_ch(const float* chs1, int C1, const float* chs2, int C2, const float* gamma, const float* beta, int B,
                     int HW, float eps, const float* emb, int emb_ld, const float* embz, int embz_ld, float* ab,
                     pdae_stream_t stream);
+/* Deterministic forms (torch.use_deterministic_algorithms): bitwise-identical results for identical inputs, no float atomics.
+ * Each CTA writes its per-channel partials to its own slot of the caller-owned workspace (no initialisation needed) and the
+ * slots are summed in a fixed order; the CTA grid follows (B, HW) only.  workspace: pdae_stats_det_workspace_bytes(B, HW, C)
+ * bytes, with C = C1 + C2 for pdae_gn_stats_det (a negative size: bad arguments).  Same outputs and shapes as pdae_ch_stats /
+ * pdae_gn_stats (C <= 6144).                                                                                                */
+int64_t pdae_stats_det_workspace_bytes(int B, int HW, int C);
+int pdae_ch_stats_det(const float* src, int B, int HW, int C, float* chs, float* workspace, int64_t workspace_bytes,
+                      pdae_stream_t stream);
+int pdae_gn_stats_det(const float* src1, int C1, const float* src2, int C2, int B, int HW, double* sums, float* workspace,
+                      int64_t workspace_bytes, pdae_stream_t stream);
 
 /* ---- attention (model/module.py:422-488) ---------------------------------------------------------
  * qkv: fp32 [B][T][3C] token-major.  legacy != 0: per-head channel blocks [q|k|v] (QKVAttentionLegacy);
@@ -241,6 +251,11 @@ int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan, const void* src1, int C1, co
                          const void* skp2, int S2, const void* w_skip, const void* residual, void* out, int out_dtype,
                          float* ch_stats, int B, int H, int W, int Cout, int bn_override);
 int pdae_conv_tc3_run(const pdae_conv_tc3_plan* plan, pdae_stream_t stream);
+/* Deterministic statistics: the DET kernel stores each 16 x 8 tile's per-channel sums in the tile's own slot and the run sums
+ * an image's slots in order into ch_stats.  Call once, after create and before the first run; workspace: caller-owned,
+ * pdae_conv_tc3_det_workspace_bytes(plan) bytes (0: one tile per image or no statistics; the slots are then ch_stats itself).  */
+int64_t pdae_conv_tc3_det_workspace_bytes(const pdae_conv_tc3_plan* plan);
+int pdae_conv_tc3_set_deterministic(pdae_conv_tc3_plan* plan, float* workspace, int64_t workspace_bytes);
 void pdae_conv_tc3_destroy(pdae_conv_tc3_plan* plan);
 
 /* Weight gradient of a stride-1 3x3 / 1x1 "same" convolution on the tensor cores (what autograd computes for conv weights
@@ -336,6 +351,13 @@ int pdae_conv_tc2_create_s2_ex(pdae_conv_tc2_plan** plan, const void* in_bf16, c
 int pdae_conv_tc2_create_splitk(pdae_conv_tc2_plan** plan, const void* in_bf16, const void* w_bf16, const float* bias, float* out,
                                 int B, int Cin, int Cout);
 int pdae_conv_tc2_run(const pdae_conv_tc2_plan* plan, pdae_stream_t stream);
+/* Deterministic plans: switch a forward conv (stride 1 or 2, with or without fused skip), a plain batched GEMM or a split-K
+ * Linear plan to the DET kernels (no float atomics).  Statistics as pdae_conv_tc3_set_deterministic.  Split-K: each (tile, k
+ * range) stores its partial tile in its own slot and the run adds the ranges in order, then the bias, into `out`, which no
+ * longer needs zeroing; the number of k ranges follows Cin and Cout only.  Call once, after create and before the first run;
+ * workspace: caller-owned, pdae_conv_tc2_det_workspace_bytes(plan) bytes (may be 0).  Other modes: PDAE_EINVAL.              */
+int64_t pdae_conv_tc2_det_workspace_bytes(const pdae_conv_tc2_plan* plan);
+int pdae_conv_tc2_set_deterministic(pdae_conv_tc2_plan* plan, float* workspace, int64_t workspace_bytes);
 /* Image-head plans (cout_valid > 0): fuse the per-step sampling update into the head's epilogue, x_t updated in place.
  * fuse_desc_device: 10 x int64 in DEVICE memory, read at run time, flags = enabled | use_grad<<1 | eps_only<<2 | ddpm<<3 |
  * interp<<4 | C<<8 | C_eps<<16; flags == 0 -> plain head.
@@ -367,6 +389,14 @@ int pdae_stem_conv_bf16(const float* x_nchw, const float* w_packed, const float*
  * same way: H, W the input size (H even, W % 8 == 0), out_bf16_nhwc [B][H/2][W/2][Cout], arguments otherwise as above.  */
 int pdae_stem_conv_s2_bf16(const float* x_nchw, const float* w_packed, const float* bias, void* out_bf16_nhwc, float* ch_stats,
                            int B, int H, int W, int Cin, int Cout, pdae_stream_t stream);
+/* Deterministic stems (stride 1: pdae_stem_conv_bf16, stride 2: pdae_stem_conv_s2_bf16): the same output, the statistics
+ * written (not added) to ch_stats through per-CTA slots summed in order.  workspace: pdae_stem_conv_det_workspace_bytes(B, H,
+ * W, Cout, stride) bytes (H, W: the input size).  Needs (9 Cin + 2 + 2 (256 / (Cout / 8))) Cout floats <= 48 KiB of shared
+ * memory.                                                                                                                    */
+int64_t pdae_stem_conv_det_workspace_bytes(int B, int H, int W, int Cout, int stride);
+int pdae_stem_conv_bf16_det(const float* x_nchw, const float* w_packed, const float* bias, void* out_bf16_nhwc, float* ch_stats,
+                            int B, int H, int W, int Cin, int Cout, int stride, float* workspace, int64_t workspace_bytes,
+                            pdae_stream_t stream);
 
 /* ---- callers either side of the hot path (SURVEY.md 8(f)) -------------------------------------------------------------
  * Fused multi-tensor Adam + EMA: replaces torch.optim.Adam.step() as configured at
@@ -437,6 +467,14 @@ int pdae_mse_per_image(const float* a, const float* b, int B, int64_t per_image,
                        pdae_stream_t stream);
 int pdae_ssim_per_image(const float* img1, const float* img2, const float* window_11x11, int B, int C, int H, int W,
                         double* workspace, float* out, pdae_stream_t stream);
+/* Deterministic per-image MSE / SSIM: every block's fp64 sum in its own workspace slot, an image's slots added in order.
+ * workspace: pdae_mse_det_workspace_bytes(B, per_image) / pdae_ssim_det_workspace_bytes(B, C, H, W) bytes.              */
+int64_t pdae_mse_det_workspace_bytes(int B, int64_t per_image);
+int pdae_mse_per_image_det(const float* a, const float* b, int B, int64_t per_image, double* workspace, int64_t workspace_bytes,
+                           float* out, pdae_stream_t stream);
+int64_t pdae_ssim_det_workspace_bytes(int B, int C, int H, int W);
+int pdae_ssim_per_image_det(const float* img1, const float* img2, const float* window_11x11, int B, int C, int H, int W,
+                            double* workspace, int64_t workspace_bytes, float* out, pdae_stream_t stream);
 
 #ifdef __cplusplus
 }

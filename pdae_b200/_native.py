@@ -63,6 +63,9 @@ _SIGS = {
                               _P]),
     "pdae_zero": (c_int, [_P, c_int64, _P]),
     "pdae_ch_stats": (c_int, [_P, c_int, c_int, c_int, _P, _P]),
+    "pdae_stats_det_workspace_bytes": (c_int64, [c_int, c_int, c_int]),
+    "pdae_ch_stats_det": (c_int, [_P, c_int, c_int, c_int, _P, _P, c_int64, _P]),
+    "pdae_gn_stats_det": (c_int, [_P, c_int, _P, c_int, c_int, c_int, _P, _P, c_int64, _P]),
     "pdae_gn_coef_ch": (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_float, _P, c_int, _P, c_int, _P, _P]),
     "pdae_attention_simt": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_timestep_embedding": (c_int, [_P, c_int, c_int, _P, _P, _P]),
@@ -116,11 +119,15 @@ _SIGS = {
     "pdae_conv_tc2_create_s2_ex": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_conv_tc2_create_splitk": (c_int, [POINTER(c_void_p), _P, _P, _P, _P, c_int, c_int, c_int]),
     "pdae_conv_tc2_run": (c_int, [_P, _P]),
+    "pdae_conv_tc2_det_workspace_bytes": (c_int64, [_P]),
+    "pdae_conv_tc2_set_deterministic": (c_int, [_P, _P, c_int64]),
     "pdae_conv_tc2_set_head_fuse": (c_int, [_P, _P]),
     "pdae_conv_tc3_supported": (c_int, [c_int, c_int, c_int, c_int]),
     "pdae_conv_tc3_create": (c_int, [POINTER(c_void_p), _P, c_int, _P, c_int, c_int, _P, c_int, _P, _P, _P, c_int, _P, c_int, _P, _P,
                                      _P, c_int, _P, c_int, c_int, c_int, c_int, c_int]),
     "pdae_conv_tc3_run": (c_int, [_P, _P]),
+    "pdae_conv_tc3_det_workspace_bytes": (c_int64, [_P]),
+    "pdae_conv_tc3_set_deterministic": (c_int, [_P, _P, c_int64]),
     "pdae_conv_tc3_destroy": (None, [_P]),
     "pdae_wgrad_tc_supported": (c_int, [c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_create": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
@@ -139,6 +146,8 @@ _SIGS = {
     "pdae_mul_mask_cols": (c_int, [_P, c_int, _P, c_float, c_int, c_int, _P]),
     "pdae_stem_conv_bf16": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
     "pdae_stem_conv_s2_bf16": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P]),
+    "pdae_stem_conv_det_workspace_bytes": (c_int64, [c_int, c_int, c_int, c_int, c_int]),
+    "pdae_stem_conv_bf16_det": (c_int, [_P, _P, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64, _P]),
     "pdae_gn_apply_split3": (c_int, [_P, c_int, _P, c_int, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int, _P]),
     "pdae_adam_ema_step": (c_int, [_P, _P, c_int, c_int, c_float, c_float, c_float, c_float, c_float, c_int64, c_float,
                                    c_float, _P]),
@@ -153,6 +162,10 @@ _SIGS = {
     "pdae_u8_nhwc_to_images": (c_int, [_P, _P, c_int, c_int, c_int, c_int, _P]),
     "pdae_mse_per_image": (c_int, [_P, _P, c_int, c_int64, _P, _P, _P]),
     "pdae_ssim_per_image": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, _P, _P]),
+    "pdae_mse_det_workspace_bytes": (c_int64, [c_int, c_int64]),
+    "pdae_mse_per_image_det": (c_int, [_P, _P, c_int, c_int64, _P, c_int64, _P, _P]),
+    "pdae_ssim_det_workspace_bytes": (c_int64, [c_int, c_int, c_int, c_int]),
+    "pdae_ssim_per_image_det": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, _P, c_int64, _P, _P]),
 }
 EXPORTS = tuple(_SIGS.keys())
 

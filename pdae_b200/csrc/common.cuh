@@ -10,6 +10,9 @@
 namespace pdae {
 
 void set_error(const char* fmt, ...);
+// Deterministic statistics (norm_elementwise.cu): per-channel (sum, sum^2) partials [B][P][C][2], written with plain stores by
+// P producers per image, summed over P in ascending order into [B][C][2].
+cudaError_t launch_stat_parts_reduce(const float* part, int B, int P, int C, float* chs, cudaStream_t s);
 
 #define PDAE_REQUIRE(cond, ...)             \
   do {                                      \

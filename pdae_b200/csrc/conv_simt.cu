@@ -231,7 +231,9 @@ __global__ void __launch_bounds__(256) conv3x3_smalln_kernel(const TIn* __restri
 // thread -> (pixel slot, channel octet); weights [27][Cout] in shared memory.
 // S = 2: the semantic encoder's stride-2 stem (encoder/ffhq.py: nn.Conv2d(3, 64, 3, 2, 1)); H, W stay the INPUT size and the
 // output is [B][H/2][W/2][Cout].  A thread's 4 output pixels read input columns 2 x0 - 1 .. 2 x0 + 7 of each row.
-template <int CIN, int S = 1>
+// DET: deterministic statistics -- no atomics: the thread partials meet in shared memory and are added in slot order, and the
+// CTA's sums go to its own slot stats[b][blockIdx.x][Cout][2] (summed over the CTAs in order by stat_parts_reduce).
+template <int CIN, int S = 1, bool DET = false>
 __global__ void __launch_bounds__(256) stem_conv_bf16_kernel(const float* __restrict__ x, const float* __restrict__ w,
                                                              const float* __restrict__ bias, __nv_bfloat16* __restrict__ out,
                                                              float* __restrict__ stats, int H, int W, int Cout) {
@@ -311,14 +313,35 @@ __global__ void __launch_bounds__(256) stem_conv_bf16_kernel(const float* __rest
       }
     }
     if (stats) {
+      if constexpr (DET) {
+        float* sp = acc + 2 * Cout + (size_t)slot * 2 * Cout;   // [ppc][2][Cout]
 #pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        atomicAdd(acc + c + j, s1[j]);
-        atomicAdd(acc + Cout + c + j, s2[j]);
+        for (int j = 0; j < 8; ++j) {
+          sp[c + j] = s1[j];
+          sp[Cout + c + j] = s2[j];
+        }
+      } else {
+#pragma unroll
+        for (int j = 0; j < 8; ++j) {
+          atomicAdd(acc + c + j, s1[j]);
+          atomicAdd(acc + Cout + c + j, s2[j]);
+        }
       }
     }
   }
-  if (stats) {
+  if constexpr (DET) {
+    if (stats) {
+      __syncthreads();
+      for (int i = threadIdx.x; i < Cout; i += 256) {
+        float a = 0.f, q = 0.f;
+        for (int k = 0; k < ppc; ++k) {
+          a += acc[2 * Cout + (size_t)k * 2 * Cout + i];
+          q += acc[2 * Cout + (size_t)k * 2 * Cout + Cout + i];
+        }
+        *reinterpret_cast<float2*>(stats + (((long long)b * gridDim.x + blockIdx.x) * Cout + i) * 2) = make_float2(a, q);
+      }
+    }
+  } else if (stats) {
     __syncthreads();
     for (int i = threadIdx.x; i < Cout; i += 256) {
       atomicAdd(stats + ((long long)b * Cout + i) * 2, acc[i]);
@@ -441,5 +464,59 @@ extern "C" int pdae_stem_conv_s2_bf16(const float* x_nchw, const float* w_packed
     default: stem_conv_bf16_kernel<4, 2><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, ch_stats, H, W, Cout); break;
   }
   PDAE_LAUNCH_CHECK("stem_conv_bf16_kernel<stride 2>");
+  return PDAE_OK;
+}
+
+// Deterministic stems: the same convs, with the statistics in fixed slots (one per CTA) summed in a fixed order.  The CTA count
+// follows (H, W, Cout, stride) only.
+static int stem_grid_x(int H, int W, int Cout, int stride) {
+  const int Ho = H / stride, Wo = W / stride, ppc = 256 / (Cout / 8);
+  int gx = cdiv((long long)Ho * (Wo / 4), (long long)ppc * 2);
+  if (gx > 148 * 8) gx = 148 * 8;
+  return gx < 1 ? 1 : gx;
+}
+
+extern "C" int64_t pdae_stem_conv_det_workspace_bytes(int B, int H, int W, int Cout, int stride) {
+  if (B <= 0 || H <= 0 || W <= 0 || Cout % 8 != 0 || Cout < 8 || Cout > 256 || (stride != 1 && stride != 2)) {
+    ::pdae::set_error("stem_conv_det_workspace_bytes: B=%d H=%d W=%d Cout=%d stride=%d unsupported", B, H, W, Cout, stride);
+    return PDAE_EINVAL;
+  }
+  return (int64_t)B * stem_grid_x(H, W, Cout, stride) * Cout * 2 * (int64_t)sizeof(float);
+}
+
+extern "C" int pdae_stem_conv_bf16_det(const float* x_nchw, const float* w_packed, const float* bias, void* out_bf16_nhwc,
+                                       float* ch_stats, int B, int H, int W, int Cin, int Cout, int stride, float* workspace,
+                                       int64_t workspace_bytes, pdae_stream_t stream) {
+  PDAE_REQUIRE(x_nchw && w_packed && out_bf16_nhwc && ch_stats && workspace, "stem_conv_bf16_det: null pointer");
+  PDAE_REQUIRE(stride == 1 || stride == 2, "stem_conv_bf16_det: stride=%d must be 1 or 2", stride);
+  PDAE_REQUIRE(B > 0 && B <= 65535, "stem_conv_bf16_det: B=%d must be in [1, 65535]", B);
+  PDAE_REQUIRE(Cin >= 1 && Cin <= 4, "stem_conv_bf16_det: Cin=%d (image channels) must be 1..4", Cin);
+  PDAE_REQUIRE(Cout % 8 == 0 && Cout >= 8 && Cout <= 256, "stem_conv_bf16_det: Cout=%d must be a multiple of 8 in [8, 256]", Cout);
+  PDAE_REQUIRE(stride == 1 ? (H > 0 && W > 0 && W % 4 == 0) : (H >= 2 && W >= 8 && H % 2 == 0 && W % 8 == 0),
+               "stem_conv_bf16_det: H=%d W=%d unsupported at stride %d", H, W, stride);
+  PDAE_REQUIRE(!(((uintptr_t)x_nchw | (uintptr_t)out_bf16_nhwc) & 15) && !(((uintptr_t)ch_stats | (uintptr_t)workspace) & 7),
+               "stem_conv_bf16_det: x and out must be 16-byte, ch_stats and workspace 8-byte aligned");
+  const int gx = stem_grid_x(H, W, Cout, stride);
+  const long long need = (long long)B * gx * Cout * 2 * (long long)sizeof(float);
+  PDAE_REQUIRE(workspace_bytes >= need, "stem_conv_bf16_det: workspace of %lld bytes, %lld needed (pdae_stem_conv_det_workspace_bytes)",
+               (long long)workspace_bytes, need);
+  const int ppc = 256 / (Cout / 8);
+  const size_t smem = (size_t)(9 * Cin + 2 + 2 * ppc) * Cout * sizeof(float);
+  PDAE_REQUIRE(smem <= 48 * 1024, "stem_conv_bf16_det: Cin=%d Cout=%d need %zu bytes of shared memory (at most 48 KiB)", Cin, Cout,
+               smem);
+  dim3 grid(gx, B);
+  cudaStream_t s = (cudaStream_t)stream;
+  __nv_bfloat16* o = (__nv_bfloat16*)out_bf16_nhwc;
+#define PDAE_STEM_DET(S)                                                                                                     \
+  switch (Cin) {                                                                                                             \
+    case 1: stem_conv_bf16_kernel<1, S, true><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, workspace, H, W, Cout); break; \
+    case 2: stem_conv_bf16_kernel<2, S, true><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, workspace, H, W, Cout); break; \
+    case 3: stem_conv_bf16_kernel<3, S, true><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, workspace, H, W, Cout); break; \
+    default: stem_conv_bf16_kernel<4, S, true><<<grid, 256, smem, s>>>(x_nchw, w_packed, bias, o, workspace, H, W, Cout); break; \
+  }
+  if (stride == 1) PDAE_STEM_DET(1) else PDAE_STEM_DET(2)
+#undef PDAE_STEM_DET
+  PDAE_LAUNCH_CHECK("stem_conv_bf16_kernel<det>");
+  PDAE_CUDA(launch_stat_parts_reduce(workspace, B, gx, Cout, ch_stats, s));
   return PDAE_OK;
 }

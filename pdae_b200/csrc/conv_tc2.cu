@@ -37,6 +37,12 @@
 // work item is (tile, k range): item = tile * splitk + split covers k-blocks [split kchunk, split kchunk + kchunk).  Each
 // item adds its partial tile into the zeroed fp32 output with red.global.add straight from the accumulator fragments
 // (rows past the batch skipped), split 0 adding the bias as well.  fp32 output only: no residual, statistics or bf16 store.
+//
+// DET: the deterministic instantiations (pdae_conv_tc2_set_deterministic) use no float atomics.  Statistics: a tile inside one
+// image stores its per-channel sums in the tile's own slot [B][tiles per image][Cout][2] (plain stores; the run then sums the
+// slots in order); a tile holding several whole images sums each (image, column) with one thread, in row order, straight into
+// [B][Cout][2].  Split-K: item (tile, split) stores its partial tile in slot [split][B][Cout] and the run adds the splits in
+// order, then the bias; the split count follows K and N alone.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -168,7 +174,7 @@ __device__ __forceinline__ void cons_bar() { asm volatile("bar.sync 1, 256;" :::
 // byte offset of (row, 16-byte chunk) inside a 128-row x 128-byte SWIZZLE_128B staging tile
 __device__ __forceinline__ uint32_t swz(int row, int chunk16) { return (uint32_t)(row * 128 + ((chunk16 ^ (row & 7)) << 4)); }
 
-template <int BN, bool OB, int S2 = 0, int GM = 0>
+template <int BN, bool OB, int S2 = 0, int GM = 0, bool DET = false>
 __global__ void __launch_bounds__(T2_THREADS, 1)
 conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB,
                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
@@ -394,6 +400,15 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
 
       if constexpr (SK) {
         // split-K partial tile (H = W = 1: tile row r is batch row b0 + r): fp32 reductions into the zeroed output
+        if constexpr (DET) {
+          float* slot = p.out_nchw + (long long)(kb0 / p.kchunk) * p.B * p.Cout;
+#pragma unroll
+          for (int i = 0; i < BN / 2; i += 2) {
+            const int b = b0 + 64 * wg + wgmma::frag_row(t, i), col = n0 + wgmma::frag_col(t, i);
+            if (b < p.B) *reinterpret_cast<float2*>(slot + (long long)b * p.Cout + col) = make_float2(acc[i], acc[i + 1]);
+          }
+          continue;
+        }
         const bool add_bias = p.bias != nullptr && kb0 == 0;
 #pragma unroll
         for (int i = 0; i < BN / 2; i += 2) {
@@ -626,7 +641,30 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               }
               return x;
             };
-            if (p.tn == 1) {
+            if (DET && p.tn != 1) {
+              // several whole images per tile: (image, column) pairs, each summed over the image's rows in order by one thread
+              for (int pr = ct; pr < p.tn * CW; pr += T2_CONSUMERS) {
+                const int img = pr / CW, cc = pr - img * CW;
+                if (b0 + img >= p.B) continue;
+                const uint32_t cb = OB ? (uint32_t)((cc & 7) * 2) : (uint32_t)((cc & 3) * 4);
+                const int ck = OB ? (cc >> 3) : (cc >> 2);
+                float sacc = 0.f, qq = 0.f;
+                for (int rr = img * ppi; rr < (img + 1) * ppi; ++rr) {
+                  float x;
+                  if (OB) {
+                    unsigned short h;
+                    asm volatile("ld.shared.u16 %0, [%1];" : "=h"(h) : "r"(obuf + swz(rr, ck) + cb));
+                    x = __uint_as_float(((uint32_t)h) << 16);
+                  } else {
+                    asm volatile("ld.shared.f32 %0, [%1];" : "=f"(x) : "r"(obuf + swz(rr, ck) + cb));
+                  }
+                  sacc += x;
+                  qq = fmaf(x, x, qq);
+                }
+                *reinterpret_cast<float2*>(p.ch_stats + ((long long)(b0 + img) * p.Cout + n0 + c * CW + cc) * 2) =
+                    make_float2(sacc, qq);
+              }
+            } else if (p.tn == 1) {
               // whole tile = one image: accumulate in shared memory across this CTA's consecutive tiles.  The row runs of a
               // column are added in a fixed order by one thread, so repeated runs give identical statistics.
               float sacc = 0.f, qq = 0.f;
@@ -647,8 +685,15 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                   s2 += part[g * CW + ct];
                   q2 += part[256 + g * CW + ct];
                 }
-                st_acc[0][c * CW + ct] += s2;
-                st_acc[1][c * CW + ct] += q2;
+                if constexpr (DET) {   // this tile's slot
+                  const int pimg = (tl - nt * p.tiles_m) % (p.tiles_x * p.tiles_y);
+                  *reinterpret_cast<float2*>(
+                      p.ch_stats + (((long long)b0 * p.tiles_x * p.tiles_y + pimg) * p.Cout + n0 + c * CW + ct) * 2) =
+                      make_float2(s2, q2);
+                } else {
+                  st_acc[0][c * CW + ct] += s2;
+                  st_acc[1][c * CW + ct] += q2;
+                }
               }
             } else if (ppi % RPT == 0) {
               // several whole images per tile and this thread's RPT rows lie inside ONE image
@@ -695,7 +740,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
             }
           }
         }
-        if (p.ch_stats && p.tn == 1) {
+        if (!DET && p.ch_stats && p.tn == 1) {
           bool flush = tile + 1 >= tile_end;
           if (!flush) {
             const int nt2 = (tile + 1) / p.tiles_m;
@@ -743,18 +788,29 @@ static int pow2_tile(int W, int cap) {
   return t;
 }
 
-template <int BN, bool OB, int S2 = 0, int GM = 0>
+template <int BN, bool OB, int S2 = 0, int GM = 0, bool DET = false>
 static cudaError_t launch_tc2(const CUtensorMap& a, const CUtensorMap& b, const CUtensorMap& o, const CUtensorMap& r,
                               const CUtensorMap& a2, const CUtensorMap& b2, const CUtensorMap& a3, const ConvTc2Args& args,
                               const SmGradArgs& sg, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, OB, S2, GM>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, stats <= 2 KB) <= 227 KB
+    cudaError_t e = cudaFuncSetAttribute(conv_tc2_kernel<BN, OB, S2, GM, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);  // + static (barriers, stats <= 2 KB) <= 227 KB
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  conv_tc2_kernel<BN, OB, S2, GM><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args, sg);
+  conv_tc2_kernel<BN, OB, S2, GM, DET><<<grid, T2_THREADS, smem, s>>>(a, b, o, r, a2, b2, a3, args, sg);
   return cudaPeekAtLastError();
+}
+
+// deterministic split-K: out[b][n] = (sum over the splits in order of part[split][b][n]) + bias[n]
+__global__ void __launch_bounds__(256) splitk_reduce_kernel(const float* __restrict__ part, int splitk, long long n, int Cout,
+                                                            const float* __restrict__ bias, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float a = part[i];
+  for (int k = 1; k < splitk; ++k) a += part[(long long)k * n + i];
+  if (bias) a += bias[i % Cout];
+  out[i] = a;
 }
 
 }  // namespace pdae
@@ -769,6 +825,8 @@ struct pdae_conv_tc2_plan {
   int s2;           // 0: stride-1 conv / GEMM; 1: stride-2 forward; 2: stride-2 data gradient (conv_tc2_kernel's S2)
   int gm;           // batched-GEMM operand / epilogue mode (conv_tc2_kernel's GM)
   size_t smem;
+  int det;          // pdae_conv_tc2_set_deterministic: the DET kernel
+  float* det_out;   // DET: where the run reduces the slots to (the [B][Cout][2] statistics or the split-K output), or nullptr
 };
 
 static int g_num_sms = 0;
@@ -1234,6 +1292,59 @@ extern "C" int pdae_conv_tc2_create_s2_dgrad(pdae_conv_tc2_plan** plan_out, cons
   return tc2_create(plan_out, d);
 }
 
+// ---- deterministic plans (kernel header, DET) ----------------------------------------------------------------------------
+constexpr int T2_DET_SPLIT_ITEMS = 128;   // split-K: about this many (n-tile, split) items per row tile, whatever the batch or GPU
+
+static int tc2_det_splitk(const pdae_conv_tc2_plan* pl, int* kchunk) {
+  const int ntn = pl->args.Cout / pl->BN;
+  const int want = ntn >= T2_DET_SPLIT_ITEMS ? 1 : T2_DET_SPLIT_ITEMS / ntn;
+  const int kc = (pl->args.kblocks + want - 1) / want;
+  if (kchunk) *kchunk = kc;
+  return (pl->args.kblocks + kc - 1) / kc;
+}
+
+static bool tc2_det_mode_ok(const pdae_conv_tc2_plan* pl) { return pl->gm == GM_SPLITK || (pl->gm == 0 && pl->s2 != 2); }
+
+extern "C" int64_t pdae_conv_tc2_det_workspace_bytes(const pdae_conv_tc2_plan* pl) {
+  if (!pl) {
+    set_error("conv_tc2_det_workspace_bytes: null plan");
+    return PDAE_EINVAL;
+  }
+  const ConvTc2Args& a = pl->args;
+  if (pl->gm == GM_SPLITK) return (int64_t)tc2_det_splitk(pl, nullptr) * a.B * a.Cout * (int64_t)sizeof(float);
+  const float* stats = pl->det ? pl->det_out : a.ch_stats;
+  if (!stats || a.tn != 1 || a.tiles_x * a.tiles_y == 1) return 0;
+  return (int64_t)a.B * a.tiles_x * a.tiles_y * a.Cout * 2 * (int64_t)sizeof(float);
+}
+
+// Switch a plan of a forward conv (stride 1 or 2), a batched GEMM without a special epilogue or a split-K Linear to the
+// deterministic kernels.  `workspace` (pdae_conv_tc2_det_workspace_bytes, owned by the caller, no initialisation needed) holds
+// the slots; the run reduces them.  A split-K plan's output no longer needs zeroing.
+extern "C" int pdae_conv_tc2_set_deterministic(pdae_conv_tc2_plan* pl, float* workspace, int64_t workspace_bytes) {
+  PDAE_REQUIRE(pl, "conv_tc2_set_deterministic: null plan");
+  PDAE_REQUIRE(!pl->det, "conv_tc2_set_deterministic: the plan is deterministic already");
+  PDAE_REQUIRE(tc2_det_mode_ok(pl), "conv_tc2_set_deterministic: mode %d (s2 %d) has no deterministic form", pl->gm, pl->s2);
+  const int64_t need = pdae_conv_tc2_det_workspace_bytes(pl);
+  PDAE_REQUIRE(workspace_bytes >= need && (need == 0 || workspace),
+               "conv_tc2_set_deterministic: workspace of %lld bytes, %lld needed (pdae_conv_tc2_det_workspace_bytes)",
+               (long long)workspace_bytes, (long long)need);
+  PDAE_REQUIRE(!((uintptr_t)workspace & 7), "conv_tc2_set_deterministic: workspace must be 8-byte aligned");
+  ConvTc2Args& a = pl->args;
+  if (pl->gm == GM_SPLITK) {
+    const int tiles = a.tiles_total / a.splitk;
+    a.splitk = tc2_det_splitk(pl, &a.kchunk);
+    a.tiles_total = tiles * a.splitk;
+    pl->grid = a.tiles_total < g_num_sms ? a.tiles_total : g_num_sms;
+    pl->det_out = a.out_nchw;
+    a.out_nchw = workspace;
+  } else if (need > 0) {
+    pl->det_out = a.ch_stats;
+    a.ch_stats = workspace;
+  }
+  pl->det = 1;
+  return PDAE_OK;
+}
+
 extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t stream) {
   PDAE_REQUIRE(pl, "conv_tc2_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
@@ -1244,7 +1355,30 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
 #define T2_GO_GM(BN, OB, GM) \
   launch_tc2<BN, OB, 0, GM>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
   const bool ob = pl->args.out_bf16 != 0;
-  if (pl->gm == GM_SPLITK) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_SPLITK) : T2_GO_GM(64, false, GM_SPLITK);
+  if (pl->det) {
+#define T2_GO_DET(BN, OB, S2, GM) \
+  launch_tc2<BN, OB, S2, GM, true>(pl->tmA, pl->tmB, pl->tmO, pl->tmR, pl->tmA2, pl->tmB2, pl->tmA3, pl->args, pl->sg, pl->grid, pl->smem, s)
+    const ConvTc2Args& a = pl->args;
+    if (pl->gm == GM_SPLITK) {
+      e = pl->BN == 128 ? T2_GO_DET(128, false, 0, GM_SPLITK) : T2_GO_DET(64, false, 0, GM_SPLITK);
+      if (e == cudaSuccess) {
+        const long long n = (long long)a.B * a.Cout;
+        splitk_reduce_kernel<<<cdiv(n, 256), 256, 0, s>>>(a.out_nchw, a.splitk, n, a.Cout, a.bias, pl->det_out);
+        e = cudaPeekAtLastError();
+      }
+    } else {
+      if (pl->s2 == 1) e = pl->BN == 128 ? (ob ? T2_GO_DET(128, true, 1, 0) : T2_GO_DET(128, false, 1, 0))
+                                         : (ob ? T2_GO_DET(64, true, 1, 0) : T2_GO_DET(64, false, 1, 0));
+      else switch (pl->BN) {
+        case 16: e = T2_GO(16, false); break;   // (the image head has no statistics)
+        case 64: e = ob ? T2_GO_DET(64, true, 0, 0) : T2_GO_DET(64, false, 0, 0); break;
+        case 128: e = ob ? T2_GO_DET(128, true, 0, 0) : T2_GO_DET(128, false, 0, 0); break;
+        default: e = ob ? T2_GO_DET(256, true, 0, 0) : T2_GO_DET(256, false, 0, 0); break;
+      }
+      if (e == cudaSuccess && pl->det_out) e = launch_stat_parts_reduce(a.ch_stats, a.B, a.tiles_x * a.tiles_y, a.Cout, pl->det_out, s);
+    }
+#undef T2_GO_DET
+  } else if (pl->gm == GM_SPLITK) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_SPLITK) : T2_GO_GM(64, false, GM_SPLITK);
   else if (pl->gm == (GM_SMGRAD | GM_SPLITN)) e = T2_GO_GM(128, true, GM_SMGRAD | GM_SPLITN);
   else if (pl->gm == GM_SMGRAD) e = pl->BN == 128 ? T2_GO_GM(128, true, GM_SMGRAD) : T2_GO_GM(64, true, GM_SMGRAD);
   else if (pl->gm == GM_A_MN) e = pl->BN == 128 ? T2_GO_GM(128, false, GM_A_MN) : T2_GO_GM(64, false, GM_A_MN);

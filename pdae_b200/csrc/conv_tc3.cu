@@ -54,7 +54,8 @@ struct ConvTc3Args {
   int S1, S2;                           // raw input of the fused 1x1 skip conv: S1 | S2 channels (tensor maps tmK1 | tmK2)
   const float* bias;
   const float* res_f32;                 // X3 only: fp32 NHWC residual read straight from global memory by the epilogue
-  float* ch_stats;                      // [B][Cout][2] (sum, sum^2) accumulators of the OUTPUT or nullptr
+  float* ch_stats;                      // [B][Cout][2] (sum, sum^2) accumulators of the OUTPUT or nullptr; DET: the slots
+                                        // [B][tiles_x * tiles_y][Cout][2], one per (image, tile of the image), plain stores
   int B, H, W, Cout;
   int tiles_x, tiles_y, tiles_m, tiles_total;
   int kblocks, kblocks2;
@@ -154,7 +155,9 @@ __device__ __forceinline__ uint32_t pack_bf16(float a, float b) {
 }
 }  // namespace t3
 
-template <int BN, bool X3, bool OB>
+// DET: deterministic statistics (pdae_conv_tc3_set_deterministic): no atomics; each tile's per-channel sums go to the tile's own
+// slot, which depends on the tile alone (not on the CTA that ran it).
+template <int BN, bool X3, bool OB, bool DET = false>
 __global__ void __launch_bounds__(T3_THREADS, 1)
 conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__ CUtensorMap tmB2,
                 const __grid_constant__ CUtensorMap tmO, const __grid_constant__ CUtensorMap tmR,
@@ -541,12 +544,18 @@ conv_tc3_kernel(const __grid_constant__ CUtensorMap tmB, const __grid_constant__
               s2 += st_part[0][g * CW + ct];
               q2 += st_part[1][g * CW + ct];
             }
-            st_acc[0][c * CW + ct] += s2;
-            st_acc[1][c * CW + ct] += q2;
+            if constexpr (DET) {
+              const int pimg = (tile - nt * p.tiles_m) % tiles_img;
+              *reinterpret_cast<float2*>(p.ch_stats + (((long long)b0 * tiles_img + pimg) * p.Cout + n0 + c * CW + ct) * 2) =
+                  make_float2(s2, q2);
+            } else {
+              st_acc[0][c * CW + ct] += s2;
+              st_acc[1][c * CW + ct] += q2;
+            }
           }
         }
       }
-      if (p.ch_stats) {
+      if (!DET && p.ch_stats) {
         bool flush = tile + 1 >= tile_end;
         if (!flush) {
           const int nt2 = (tile + 1) / p.tiles_m;
@@ -587,16 +596,16 @@ static EncodeTiledFn3 encode_fn3() {
   return fn;
 }
 
-template <int BN, bool X3, bool OB>
+template <int BN, bool X3, bool OB, bool DET = false>
 static cudaError_t launch_tc3(const CUtensorMap& b, const CUtensorMap& b2, const CUtensorMap& o, const CUtensorMap& r,
                               const CUtensorMap* sk, const ConvTc3Args& args, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(conv_tc3_kernel<BN, X3, OB>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(conv_tc3_kernel<BN, X3, OB, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  conv_tc3_kernel<BN, X3, OB><<<grid, T3_THREADS, smem, s>>>(b, b2, o, r, sk[0], sk[1], sk[2], sk[3], args);
+  conv_tc3_kernel<BN, X3, OB, DET><<<grid, T3_THREADS, smem, s>>>(b, b2, o, r, sk[0], sk[1], sk[2], sk[3], args);
   return cudaPeekAtLastError();
 }
 
@@ -610,6 +619,8 @@ struct pdae_conv_tc3_plan {
   ConvTc3Args args;
   int BN, x3, grid;
   size_t smem;
+  int det;              // pdae_conv_tc3_set_deterministic: the DET kernel
+  float* det_stats;     // DET with several tiles per image: the [B][Cout][2] sums the slots are reduced into (else nullptr)
 };
 
 static int g_num_sms3 = 0;
@@ -758,14 +769,51 @@ extern "C" int pdae_conv_tc3_create(pdae_conv_tc3_plan** plan_out, const void* s
   return PDAE_OK;
 }
 
+// Deterministic statistics: the tiles' per-channel sums go to fixed slots [B][P][Cout][2] (P = tiles per image) in `workspace`
+// and are summed over P in order into the plan's ch_stats by the same run.  With one tile per image the slots ARE ch_stats and
+// no workspace is needed.  Without statistics the DET kernel is the default one, and nothing changes.
+static int tc3_tiles_img(const pdae_conv_tc3_plan* pl) { return pl->args.tiles_x * pl->args.tiles_y; }
+
+extern "C" int64_t pdae_conv_tc3_det_workspace_bytes(const pdae_conv_tc3_plan* pl) {
+  if (!pl) {
+    set_error("conv_tc3_det_workspace_bytes: null plan");
+    return PDAE_EINVAL;
+  }
+  const float* stats = pl->det ? pl->det_stats : pl->args.ch_stats;
+  const int P = tc3_tiles_img(pl);
+  if (!stats || P == 1) return 0;
+  return (int64_t)pl->args.B * P * pl->args.Cout * 2 * (int64_t)sizeof(float);
+}
+
+extern "C" int pdae_conv_tc3_set_deterministic(pdae_conv_tc3_plan* pl, float* workspace, int64_t workspace_bytes) {
+  PDAE_REQUIRE(pl, "conv_tc3_set_deterministic: null plan");
+  PDAE_REQUIRE(!pl->det, "conv_tc3_set_deterministic: the plan is deterministic already");
+  const int64_t need = pdae_conv_tc3_det_workspace_bytes(pl);
+  PDAE_REQUIRE(workspace_bytes >= need && (need == 0 || workspace),
+               "conv_tc3_set_deterministic: workspace of %lld bytes, %lld needed (pdae_conv_tc3_det_workspace_bytes)",
+               (long long)workspace_bytes, (long long)need);
+  PDAE_REQUIRE(!((uintptr_t)workspace & 7), "conv_tc3_set_deterministic: workspace must be 8-byte aligned");
+  pl->det = 1;
+  if (need > 0) {
+    pl->det_stats = pl->args.ch_stats;
+    pl->args.ch_stats = workspace;
+  }
+  return PDAE_OK;
+}
+
 extern "C" int pdae_conv_tc3_run(const pdae_conv_tc3_plan* pl, pdae_stream_t stream) {
   PDAE_REQUIRE(pl, "conv_tc3_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
-#define T3_GO(BN, X3) (pl->args.out_bf16 ? launch_tc3<BN, X3, true>(pl->tmB, pl->tmB2, pl->tmO, pl->tmR, pl->tmS, pl->args, pl->grid, pl->smem, s) \
-                                         : launch_tc3<BN, X3, false>(pl->tmB, pl->tmB2, pl->tmO, pl->tmR, pl->tmS, pl->args, pl->grid, pl->smem, s))
-  if (pl->x3) e = pl->BN == 64 ? T3_GO(64, true) : T3_GO(128, true);
-  else e = pl->BN == 64 ? T3_GO(64, false) : T3_GO(128, false);
+#define T3_GO(BN, X3, D) (pl->args.out_bf16 ? launch_tc3<BN, X3, true, D>(pl->tmB, pl->tmB2, pl->tmO, pl->tmR, pl->tmS, pl->args, pl->grid, pl->smem, s) \
+                                            : launch_tc3<BN, X3, false, D>(pl->tmB, pl->tmB2, pl->tmO, pl->tmR, pl->tmS, pl->args, pl->grid, pl->smem, s))
+  if (pl->det) {
+    if (pl->x3) e = pl->BN == 64 ? T3_GO(64, true, true) : T3_GO(128, true, true);
+    else e = pl->BN == 64 ? T3_GO(64, false, true) : T3_GO(128, false, true);
+    if (e == cudaSuccess && pl->det_stats)
+      e = launch_stat_parts_reduce(pl->args.ch_stats, pl->args.B, tc3_tiles_img(pl), pl->args.Cout, pl->det_stats, s);
+  } else if (pl->x3) e = pl->BN == 64 ? T3_GO(64, true, false) : T3_GO(128, true, false);
+  else e = pl->BN == 64 ? T3_GO(64, false, false) : T3_GO(128, false, false);
 #undef T3_GO
   if (e != cudaSuccess) {
     (void)cudaGetLastError();

@@ -102,6 +102,93 @@ __global__ void __launch_bounds__(256) ch_stats_kernel(const float* __restrict__
   }
 }
 
+// ---- deterministic statistics: no float atomics; every partial has a fixed slot, and slots are summed in a fixed order ----
+// Per-CTA per-channel (sum, sum^2) of a virtual concat [s1 (C1) | s2 (C2)] into part[b][blockIdx.x][C][2]: the thread partials
+// of ch_stats_kernel, combined across the CTA's pixel rows in row order through shared memory.
+__global__ void __launch_bounds__(256) ch_parts_kernel(const float* __restrict__ s1, int C1, const float* __restrict__ s2, int C2,
+                                                       int HW, float* __restrict__ part, int ppc) {
+  extern __shared__ float sh[];  // [R][2][C]
+  const int C = C1 + C2, L = C >> 2;
+  const int Lb = L < 256 ? L : 256;
+  const int R = 256 / Lb;
+  const int tid = threadIdx.x;
+  const int lane = tid % Lb, row = tid / Lb;
+  const int b = blockIdx.y;
+  const int p0 = blockIdx.x * ppc;
+  const int p1 = min(HW, p0 + ppc);
+  if (row < R) {
+    for (int cq = lane; cq < L; cq += Lb) {
+      const int c = cq * 4;
+      const float* base;
+      int cs, cc;
+      if (c < C1) { base = s1; cs = C1; cc = c; } else { base = s2; cs = C2; cc = c - C1; }
+      base += (long long)b * HW * cs + cc;
+      float4 s = make_float4(0.f, 0.f, 0.f, 0.f), q = s;
+      for (int p = p0 + row; p < p1; p += R) {
+        const float4 v = *reinterpret_cast<const float4*>(base + (long long)p * cs);
+        s.x += v.x; s.y += v.y; s.z += v.z; s.w += v.w;
+        q.x = fmaf(v.x, v.x, q.x); q.y = fmaf(v.y, v.y, q.y); q.z = fmaf(v.z, v.z, q.z); q.w = fmaf(v.w, v.w, q.w);
+      }
+      *reinterpret_cast<float4*>(sh + (size_t)row * 2 * C + c) = s;
+      *reinterpret_cast<float4*>(sh + (size_t)row * 2 * C + C + c) = q;
+    }
+  }
+  __syncthreads();
+  for (int c = tid; c < C; c += 256) {
+    float s = 0.f, q = 0.f;
+    for (int r = 0; r < R; ++r) {
+      s += sh[(size_t)r * 2 * C + c];
+      q += sh[(size_t)r * 2 * C + C + c];
+    }
+    *reinterpret_cast<float2*>(part + (((long long)b * gridDim.x + blockIdx.x) * C + c) * 2) = make_float2(s, q);
+  }
+}
+
+// part [B][P][C][2] -> chs [B][C][2].  Block = 32 channels x 8 partial lanes; lane r sums partials r, r + 8, ... in order, then
+// lane 0 adds the 8 lane sums in order: the same sums for every grid and every run.
+__global__ void __launch_bounds__(256) stat_parts_reduce_kernel(const float* __restrict__ part, int P, int C,
+                                                                float* __restrict__ chs) {
+  __shared__ float2 red[8][32];
+  const int cl = threadIdx.x & 31, r = threadIdx.x >> 5;
+  const int c = blockIdx.x * 32 + cl, b = blockIdx.y;
+  float2 a = make_float2(0.f, 0.f);
+  if (c < C) {
+    for (int p = r; p < P; p += 8) {
+      const float2 v = *reinterpret_cast<const float2*>(part + (((long long)b * P + p) * C + c) * 2);
+      a.x += v.x; a.y += v.y;
+    }
+  }
+  red[r][cl] = a;
+  __syncthreads();
+  if (r == 0 && c < C) {
+    float2 t = red[0][cl];
+    for (int k = 1; k < 8; ++k) { t.x += red[k][cl].x; t.y += red[k][cl].y; }
+    *reinterpret_cast<float2*>(chs + ((long long)b * C + c) * 2) = t;
+  }
+}
+
+cudaError_t launch_stat_parts_reduce(const float* part, int B, int P, int C, float* chs, cudaStream_t s) {
+  stat_parts_reduce_kernel<<<dim3(cdiv(C, 32), B), 256, 0, s>>>(part, P, C, chs);
+  return cudaPeekAtLastError();
+}
+
+// part [B][P][C][2] -> per-group fp64 sums [B][32][2] (gn_stats' form).  One block per image: thread (group, which, lane k)
+// sums partials k, k + 4, ... over the group's channels in order, then four lane sums are added in order.
+__global__ void __launch_bounds__(256) gn_group_reduce_kernel(const float* __restrict__ part, int P, int C,
+                                                              double* __restrict__ sums) {
+  __shared__ double red[4][64];
+  const int gw = threadIdx.x & 63, k = threadIdx.x >> 6;
+  const int g = gw & 31, which = gw >> 5, cpg = C / 32, b = blockIdx.x;
+  double a = 0.0;
+  for (int p = k; p < P; p += 4) {
+    const float* row = part + (((long long)b * P + p) * C + g * cpg) * 2 + which;
+    for (int j = 0; j < cpg; ++j) a += (double)row[2 * j];
+  }
+  red[k][gw] = a;
+  __syncthreads();
+  if (k == 0) sums[((long long)b * 32 + g) * 2 + which] = ((red[0][gw] + red[1][gw]) + red[2][gw]) + red[3][gw];
+}
+
 // GroupNorm coefficients from per-channel sums of a virtual concat [chs1 (C1) | chs2 (C2)]
 __global__ void gn_coef_ch_kernel(const float* __restrict__ chs1, int C1, const float* __restrict__ chs2, int C2,
                                   const float* __restrict__ gamma, const float* __restrict__ beta, int HW, float eps,
@@ -798,6 +885,58 @@ extern "C" int pdae_gn_coef_ch(const float* chs1, int C1, const float* chs2, int
   gn_coef_ch_kernel<<<B, C < 1024 ? (C < 64 ? 64 : C) : 1024, 0, (cudaStream_t)stream>>>(chs1, C1, chs2, C2, gamma, beta, HW,
                                                                                           eps, emb, emb_ld, embz, embz_ld, ab);
   PDAE_LAUNCH_CHECK("gn_coef_ch_kernel");
+  return PDAE_OK;
+}
+
+// Deterministic forms of pdae_ch_stats / pdae_gn_stats: per-CTA partials in the caller's workspace, summed in a fixed order.
+// The CTA count follows (B, HW) only (stats_ppc), so the workspace size does too.
+extern "C" int64_t pdae_stats_det_workspace_bytes(int B, int HW, int C) {
+  if (B <= 0 || HW <= 0 || C <= 0) {
+    ::pdae::set_error("stats_det_workspace_bytes: B=%d HW=%d C=%d must be > 0", B, HW, C);
+    return PDAE_EINVAL;
+  }
+  return (int64_t)B * cdiv(HW, stats_ppc(B, HW)) * C * 2 * (int64_t)sizeof(float);
+}
+
+static int launch_ch_parts(const char* fn, const float* src1, int C1, const float* src2, int C2, int B, int HW, float* ws,
+                           int64_t ws_bytes, cudaStream_t s, int* P_out) {
+  const int C = C1 + C2;
+  PDAE_REQUIRE(B > 0 && HW > 0, "%s: B=%d HW=%d must be > 0", fn, B, HW);
+  PDAE_REQUIRE(C1 % 4 == 0 && C2 % 4 == 0 && C > 0 && C <= 6144, "%s: C1=%d C2=%d unsupported", fn, C1, C2);
+  const int ppc = stats_ppc(B, HW), P = cdiv(HW, ppc);
+  const long long need = (long long)B * P * C * 2 * (long long)sizeof(float);
+  PDAE_REQUIRE(ws_bytes >= need, "%s: workspace of %lld bytes, %lld needed (pdae_stats_det_workspace_bytes)", fn,
+               (long long)ws_bytes, need);
+  const int L = C / 4, Lb = L < 256 ? L : 256;
+  const size_t smem = (size_t)(256 / Lb) * 2 * C * sizeof(float);
+  ch_parts_kernel<<<dim3(P, B), 256, smem, s>>>(src1, C1, src2, C2, HW, ws, ppc);
+  PDAE_LAUNCH_CHECK("ch_parts_kernel");
+  *P_out = P;
+  return PDAE_OK;
+}
+
+extern "C" int pdae_ch_stats_det(const float* src, int B, int HW, int C, float* chs, float* workspace, int64_t workspace_bytes,
+                                 pdae_stream_t stream) {
+  PDAE_REQUIRE(src && chs && workspace, "ch_stats_det: null pointer");
+  cudaStream_t s = (cudaStream_t)stream;
+  int P = 0;
+  const int rc = launch_ch_parts("ch_stats_det", src, C, nullptr, 0, B, HW, workspace, workspace_bytes, s, &P);
+  if (rc != PDAE_OK) return rc;
+  PDAE_CUDA(launch_stat_parts_reduce(workspace, B, P, C, chs, s));
+  return PDAE_OK;
+}
+
+extern "C" int pdae_gn_stats_det(const float* src1, int C1, const float* src2, int C2, int B, int HW, double* sums,
+                                 float* workspace, int64_t workspace_bytes, pdae_stream_t stream) {
+  PDAE_REQUIRE(src1 && sums && workspace, "gn_stats_det: null pointer");
+  if (!src2) C2 = 0;
+  PDAE_REQUIRE((C1 + C2) % 32 == 0, "gn_stats_det: C1=%d C2=%d: C %% 32 != 0", C1, C2);
+  cudaStream_t s = (cudaStream_t)stream;
+  int P = 0;
+  const int rc = launch_ch_parts("gn_stats_det", src1, C1, src2, C2, B, HW, workspace, workspace_bytes, s, &P);
+  if (rc != PDAE_OK) return rc;
+  gn_group_reduce_kernel<<<B, 256, 0, s>>>(workspace, P, C1 + C2, sums);
+  PDAE_LAUNCH_CHECK("gn_group_reduce_kernel");
   return PDAE_OK;
 }
 

@@ -104,7 +104,9 @@ __global__ void __launch_bounds__(256) u8_to_images_kernel(const uint8_t* __rest
 }
 
 // ---------------------------------------------------------------------------------------------
-// per-image mean squared error (metric/utils.py:62-63), fp64 accumulation
+// per-image mean squared error (metric/utils.py:62-63), fp64 accumulation.  DET: each block stores its sum in its own slot
+// acc[image][blockIdx.x] instead of adding it atomically (finish_parts_kernel adds the slots in order).
+template <bool DET = false>
 __global__ void __launch_bounds__(256) mse_kernel(const float* __restrict__ a, const float* __restrict__ b, long long per_image,
                                                   double* __restrict__ acc) {
   const long long base = (long long)blockIdx.y * per_image;
@@ -120,7 +122,8 @@ __global__ void __launch_bounds__(256) mse_kernel(const float* __restrict__ a, c
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int w = 0; w < 8; ++w) t += red[w];
-    atomicAdd(acc + blockIdx.y, t);
+    if (DET) acc[(long long)blockIdx.y * gridDim.x + blockIdx.x] = t;
+    else atomicAdd(acc + blockIdx.y, t);
   }
 }
 
@@ -129,9 +132,21 @@ __global__ void finish_mean_kernel(const double* __restrict__ acc, float* __rest
   if (i < B) out[i] = (float)(acc[i] * inv_n);
 }
 
+// the nparts slots of image i, added in slot order
+__global__ void finish_parts_kernel(const double* __restrict__ acc, long long nparts, float* __restrict__ out, int B,
+                                    double inv_n) {
+  const int i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= B) return;
+  double t = 0.0;
+  for (long long k = 0; k < nparts; ++k) t += acc[(long long)i * nparts + k];
+  out[i] = (float)(t * inv_n);
+}
+
 // SSIM (metric/utils.py:35-56): 11x11 Gaussian window (sigma 1.5, outer product of the normalised 1-D window, fp32),
 // zero padding 5, depthwise; C1 = 0.01^2, C2 = 0.03^2; mean over (C,H,W).  One CTA = one 16x16 tile of one (b,c) plane.
+// DET: each CTA stores its sum in its own slot acc[plane][tile y][tile x]; an image's slots are contiguous.
 constexpr int SSIM_T = 16, SSIM_R = 5, SSIM_S = SSIM_T + 2 * SSIM_R;
+template <bool DET = false>
 __global__ void __launch_bounds__(256) ssim_kernel(const float* __restrict__ img1, const float* __restrict__ img2,
                                                    const float* __restrict__ win2d, int C, int H, int W,
                                                    double* __restrict__ acc) {
@@ -174,7 +189,8 @@ __global__ void __launch_bounds__(256) ssim_kernel(const float* __restrict__ img
   if (threadIdx.x == 0) {
     double t = 0.0;
     for (int w = 0; w < 8; ++w) t += red[w];
-    atomicAdd(acc + b, t);
+    if (DET) acc[((long long)plane * gridDim.y + blockIdx.y) * gridDim.x + blockIdx.x] = t;
+    else atomicAdd(acc + b, t);
   }
 }
 
@@ -259,7 +275,7 @@ extern "C" int pdae_mse_per_image(const float* a, const float* b, int B, int64_t
   PDAE_CUDA(cudaMemsetAsync(workspace, 0, sizeof(double) * B, s));
   int gx = cdiv(per_image, 256 * 8);
   if (gx > 64) gx = 64;
-  mse_kernel<<<dim3(gx, B), 256, 0, s>>>(a, b, per_image, workspace);
+  mse_kernel<false><<<dim3(gx, B), 256, 0, s>>>(a, b, per_image, workspace);
   PDAE_LAUNCH_CHECK("mse_kernel");
   finish_mean_kernel<<<cdiv(B, 256), 256, 0, s>>>(workspace, out, B, 1.0 / (double)per_image);
   PDAE_LAUNCH_CHECK("finish_mean_kernel");
@@ -272,9 +288,63 @@ extern "C" int pdae_ssim_per_image(const float* img1, const float* img2, const f
   PDAE_REQUIRE((long long)B * C <= 65535, "ssim_per_image: B*C=%lld exceeds the grid z limit", (long long)B * C);
   cudaStream_t s = (cudaStream_t)stream;
   PDAE_CUDA(cudaMemsetAsync(workspace, 0, sizeof(double) * B, s));
-  ssim_kernel<<<dim3(cdiv(W, SSIM_T), cdiv(H, SSIM_T), B * C), 256, 0, s>>>(img1, img2, window_11x11, C, H, W, workspace);
+  ssim_kernel<false><<<dim3(cdiv(W, SSIM_T), cdiv(H, SSIM_T), B * C), 256, 0, s>>>(img1, img2, window_11x11, C, H, W, workspace);
   PDAE_LAUNCH_CHECK("ssim_kernel");
   finish_mean_kernel<<<cdiv(B, 256), 256, 0, s>>>(workspace, out, B, 1.0 / ((double)C * H * W));
   PDAE_LAUNCH_CHECK("finish_mean_kernel");
+  return PDAE_OK;
+}
+
+// Deterministic per-image MSE / SSIM: every block's sum has its own workspace slot, and an image's slots are added in order.
+static inline int mse_blocks(int64_t per_image) {
+  const int gx = cdiv(per_image, 256 * 8);
+  return gx > 64 ? 64 : gx;
+}
+
+extern "C" int64_t pdae_mse_det_workspace_bytes(int B, int64_t per_image) {
+  if (B <= 0 || per_image <= 0) {
+    ::pdae::set_error("mse_det_workspace_bytes: B=%d per_image=%lld must be > 0", B, (long long)per_image);
+    return PDAE_EINVAL;
+  }
+  return (int64_t)B * mse_blocks(per_image) * (int64_t)sizeof(double);
+}
+
+extern "C" int pdae_mse_per_image_det(const float* a, const float* b, int B, int64_t per_image, double* workspace,
+                                      int64_t workspace_bytes, float* out, pdae_stream_t stream) {
+  PDAE_REQUIRE(a && b && workspace && out && B > 0 && B <= 65535 && per_image > 0, "mse_per_image_det: bad args");
+  const int gx = mse_blocks(per_image);
+  const long long need = (long long)B * gx * (long long)sizeof(double);
+  PDAE_REQUIRE(workspace_bytes >= need, "mse_per_image_det: workspace of %lld bytes, %lld needed (pdae_mse_det_workspace_bytes)",
+               (long long)workspace_bytes, need);
+  cudaStream_t s = (cudaStream_t)stream;
+  mse_kernel<true><<<dim3(gx, B), 256, 0, s>>>(a, b, per_image, workspace);
+  PDAE_LAUNCH_CHECK("mse_kernel<det>");
+  finish_parts_kernel<<<cdiv(B, 256), 256, 0, s>>>(workspace, gx, out, B, 1.0 / (double)per_image);
+  PDAE_LAUNCH_CHECK("finish_parts_kernel");
+  return PDAE_OK;
+}
+
+extern "C" int64_t pdae_ssim_det_workspace_bytes(int B, int C, int H, int W) {
+  if (B <= 0 || C <= 0 || H <= 0 || W <= 0) {
+    ::pdae::set_error("ssim_det_workspace_bytes: B=%d C=%d H=%d W=%d must be > 0", B, C, H, W);
+    return PDAE_EINVAL;
+  }
+  return (int64_t)B * C * cdiv(H, SSIM_T) * cdiv(W, SSIM_T) * (int64_t)sizeof(double);
+}
+
+extern "C" int pdae_ssim_per_image_det(const float* img1, const float* img2, const float* window_11x11, int B, int C, int H, int W,
+                                       double* workspace, int64_t workspace_bytes, float* out, pdae_stream_t stream) {
+  PDAE_REQUIRE(img1 && img2 && window_11x11 && workspace && out && B > 0 && C > 0 && H > 0 && W > 0,
+               "ssim_per_image_det: bad args");
+  PDAE_REQUIRE((long long)B * C <= 65535, "ssim_per_image_det: B*C=%lld exceeds the grid z limit", (long long)B * C);
+  const long long parts = (long long)C * cdiv(H, SSIM_T) * cdiv(W, SSIM_T);
+  PDAE_REQUIRE(workspace_bytes >= (long long)B * parts * (long long)sizeof(double),
+               "ssim_per_image_det: workspace of %lld bytes, %lld needed (pdae_ssim_det_workspace_bytes)", (long long)workspace_bytes,
+               (long long)B * parts * (long long)sizeof(double));
+  cudaStream_t s = (cudaStream_t)stream;
+  ssim_kernel<true><<<dim3(cdiv(W, SSIM_T), cdiv(H, SSIM_T), B * C), 256, 0, s>>>(img1, img2, window_11x11, C, H, W, workspace);
+  PDAE_LAUNCH_CHECK("ssim_kernel<det>");
+  finish_parts_kernel<<<cdiv(B, 256), 256, 0, s>>>(workspace, parts, out, B, 1.0 / ((double)C * H * W));
+  PDAE_LAUNCH_CHECK("finish_parts_kernel");
   return PDAE_OK;
 }

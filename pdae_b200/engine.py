@@ -14,6 +14,11 @@ Precision modes
     embeddings and the DDIM update stay fp32.
   * ``bf16x3``: the same tensor-core kernels on split operands (a = hi + lo, three bf16 products per term)
     for fp32-grade results; the residual stream and GroupNorm inputs stay fp32.
+
+Deterministic plans (``Plan(..., deterministic=True)``; the modules record them while
+``torch.are_deterministic_algorithms_enabled()``): every cross-CTA reduction -- GroupNorm statistics, split-K Linears -- runs
+on kernels without float atomics whose partial results have fixed slots summed in a fixed order, so a replay gives the same
+bits for the same inputs.  The default plans keep the atomic kernels.
 """
 from __future__ import annotations
 
@@ -128,7 +133,8 @@ class CoefSpec:
 
 
 class Plan:
-    def __init__(self, device: torch.device, precision: Optional[str] = None, check_device: bool = True):
+    def __init__(self, device: torch.device, precision: Optional[str] = None, check_device: bool = True,
+                 deterministic: bool = False):
         if check_device:  # False only in CPU unit tests of the recording / buffer-assignment logic (a plan cannot run there)
             _native.require_device()
         self.device = device
@@ -141,6 +147,9 @@ class Plan:
         # bandwidth-bound top-level layers.  "bf16" precision only.
         self.stream_bf16 = self.precision == "bf16"
         self.L = _native.lib()
+        self.det = bool(deterministic)   # record the deterministic kernels (module docstring)
+        self._det_handles: list = []     # (op index, set_deterministic, workspace query, handle): DET_OPS, switched at finalize
+        self._det_ws = None
         self.ops: List[Tuple[str, list]] = []
         # ops recorded inside `with P.prologue():` depend only on inputs that are constant over a sampling loop (z):
         # a loop runs them once (run_prologue) and replays the remaining ops per step (run(prologue=False))
@@ -295,8 +304,17 @@ class Plan:
                 b._block = blk  # type: ignore[attr-defined]
             for b in ends.get(i, []):
                 free.append(b._block)  # type: ignore[attr-defined]
+        if self.det:
+            bad = sorted({fn for fn, _ in self.ops} & NONDET_OPS)
+            if bad:
+                raise ValueError(f"a deterministic plan cannot record {bad}: their kernels reduce with float atomics")
         compiled = []
         for fn, args in self.ops:
+            if self.det and fn in DET_OPS:   # the handle each of these ops compiles to is switched to its DET kernels below
+                tc3 = fn == "conv_tc3"
+                self._det_handles.append((len(compiled),
+                                          self.L.pdae_conv_tc3_set_deterministic if tc3 else self.L.pdae_conv_tc2_set_deterministic,
+                                          self.L.pdae_conv_tc3_det_workspace_bytes if tc3 else self.L.pdae_conv_tc2_det_workspace_bytes))
             if fn == "conv_tc2":
                 compiled.append(self._compile_tc2(args))
                 continue
@@ -336,6 +354,19 @@ class Plan:
                 else:
                     cargs.append(self._resolve(a))
             compiled.append((getattr(self.L, "pdae_" + fn), cargs, sidx, fn))
+        extra = {}   # op index -> launches a deterministic op adds (the reduction of its slots)
+        if self._det_handles:
+            # one workspace serves every tensor-core op of the plan: each op's slots live only inside its own run, and the ops run
+            # one after another on one stream
+            self._det_handles = [(i, st, q, compiled[i][1][0]) for i, st, q in self._det_handles]
+            need = [int(q(h)) for _, _, q, h in self._det_handles]
+            if min(need) < 0:
+                _native.check(min(need), "det_workspace_bytes")
+            self._det_ws = torch.empty(max(max(need), 16), dtype=torch.uint8, device=self.device)
+            for (i, setter, _, h), n in zip(self._det_handles, need):
+                _native.check(setter(h, ctypes.c_void_p(self._det_ws.data_ptr()), ctypes.c_int64(self._det_ws.numel())),
+                              setter.__name__)
+                extra[i] = 1 if (n > 0 or self.ops[i][0] == "conv_tc2_splitk") else 0
         self._compiled = compiled
         self._pro_idx = [i for i, p in enumerate(self.op_pro) if p]
         self._main_idx = [i for i, p in enumerate(self.op_pro) if not p]
@@ -347,7 +378,8 @@ class Plan:
         for b in self.bufs:  # a recycled buffer must not carry data from the prologue into the per-step ops
             if b.first is not None and not b.keep and not b.fixed and self.op_pro[b.first] and not self.op_pro[b.last]:
                 raise AssertionError(f"plan buffer {b.name!r} crosses the prologue boundary but is not `keep`")
-        self.n_launch = sum(_LAUNCHES.get(fn, 1) for (fn, _), p in zip(self.ops, self.op_pro) if not p)
+        self.n_launch = sum(_LAUNCHES.get(fn, 1) + extra.get(i, 0) for i, ((fn, _), p) in enumerate(zip(self.ops, self.op_pro))
+                            if not p)
         return self
 
     @staticmethod
@@ -841,6 +873,13 @@ class Plan:
         flops: the algorithmic FLOPs to record (a split-operand x / wp hold three bf16 blocks per logical channel)."""
         assert Cin % 64 == 0 and Cout % 64 == 0, (Cin, Cout)
         fl = 2.0 * B * Cin * Cout if flops is None else flops
+        if self.det:
+            # deterministic split-K at every batch size: its k ranges follow Cin and Cout alone, so a row's bits do not depend
+            # on how many rows the GEMM has (the latent loop's one-row bank GEMM equals the B-row one); no zeroing needed
+            if out is None:
+                out = self.new((B, Cout), torch.float32, name)
+            self.call("conv_tc2_splitk", x, wp, bias, out, B, Cin, Cout, flops=fl)
+            return out
         tiles = -(-B // 128) * (Cout // (128 if Cout % 128 == 0 else 64))   # = conv_tc2's output tiles
         if tiles < torch.cuda.get_device_properties(self.device).multi_processor_count:
             if out is None:
@@ -902,8 +941,11 @@ class Plan:
             return torch.bfloat16
         return torch.float32
 
-    def new_stats(self, B: int, C: int) -> "BufView":
-        """A [B][C][2] fp32 accumulator inside the plan's statistics arena (ONE memset per replay zeroes them all)."""
+    def new_stats(self, B: int, C: int):
+        """A [B][C][2] fp32 accumulator inside the plan's statistics arena (ONE memset per replay zeroes them all).  A
+        deterministic plan's kernels write their statistics instead of adding them: a plain arena buffer, no memset."""
+        if self.det:
+            return self.new((B, C, 2), torch.float32, "chs")
         off = self._stats_elems
         self._stats_elems += B * C * 2
         return BufView(self._stats_arena, off)
@@ -911,8 +953,38 @@ class Plan:
     def ch_stats(self, src: Buf, C: int, *, B, HW) -> Buf:
         """Per-channel (sum, sum^2) of an fp32 NHWC tensor that no conv epilogue produced."""
         chs = self.new((B, C, 2), torch.float32, "chs")
+        if self.det:
+            ws = self._det_workspace(B, HW, C)
+            self.call("ch_stats_det", src, B, HW, C, chs, ws, ctypes.c_int64(ws.nbytes), _STREAM)
+            return chs
         self.call("ch_stats", src, B, HW, C, chs, _STREAM)
         return chs
+
+    def _det_workspace(self, B: int, HW: int, C: int) -> Buf:
+        """Arena scratch for the per-CTA slots of ch_stats_det / gn_stats_det."""
+        n = int(self.L.pdae_stats_det_workspace_bytes(B, HW, C))
+        _native.check(min(n, 0), "pdae_stats_det_workspace_bytes")
+        return self.new((max(n, 16) // 4,), torch.float32, "stats_slots")
+
+    def stem_conv_bf16(self, x_in: Buf, wp: Buf, bias: Optional[torch.Tensor], out: Buf, *, B, H, W, Cin, Cout, stride,
+                       flops: float):
+        """The CUDA-core stem (stride 1 or 2) writing the bf16 stream and the first GroupNorm's [B][Cout][2] statistics;
+        returns the statistics buffer."""
+        st = self.new_stats(B, Cout)
+        if self.det:
+            n = int(self.L.pdae_stem_conv_det_workspace_bytes(B, H, W, Cout, stride))
+            _native.check(min(n, 0), "pdae_stem_conv_det_workspace_bytes")
+            ws = self.new((max(n, 16) // 4,), torch.float32, "stem_slots")
+            self.call("stem_conv_bf16_det", x_in, wp, self.param(bias), out, st, B, H, W, Cin, Cout, stride, ws,
+                      ctypes.c_int64(ws.nbytes), _STREAM, flops=flops)
+        else:
+            self.call("stem_conv_bf16" if stride == 1 else "stem_conv_s2_bf16", x_in, wp, self.param(bias), out, st, B, H, W,
+                      Cin, Cout, _STREAM, flops=flops)
+        return st
+
+    def stem_det_fits(self, Cin: int, Cout: int) -> bool:
+        """The deterministic stem keeps its per-thread statistics in shared memory (include/pdae_b200.h)."""
+        return not self.det or (9 * Cin + 2 + 2 * (256 // (Cout // 8))) * Cout * 4 <= 48 * 1024
 
     @property
     def fused_stats(self) -> bool:
@@ -944,7 +1016,11 @@ class Plan:
         ab = self.new((B, 2, C), torch.float32, "gn_ab")
         sums = self.new((B, 32, 2), torch.float64, "gn_sums")
         self.last_sums = sums
-        self.call("gn_stats", src1, C1, src2, C2, B, HW, sums, _STREAM)
+        if self.det:
+            ws = self._det_workspace(B, HW, C)
+            self.call("gn_stats_det", src1, C1, src2, C2, B, HW, sums, ws, ctypes.c_int64(ws.nbytes), _STREAM)
+        else:
+            self.call("gn_stats", src1, C1, src2, C2, B, HW, sums, _STREAM)
         self.call("gn_coef", sums, self.param(gamma), self.param(beta), B, C, HW, ctypes.c_float(1e-5), emb, emb_ld, embz,
                   embz_ld, ab, _STREAM)
         return ab
@@ -981,4 +1057,13 @@ class Plan:
         return act, raw
 
 
-_LAUNCHES = {"gn_stats": 1, "attention_simt": 3, "zero": 0}
+# Tensor-core ops a deterministic plan switches to their DET kernels at finalize (pdae_conv_tc2/tc3_set_deterministic).
+DET_OPS = frozenset({"conv_tc2", "conv_tc2_skip", "conv_tc2_s2", "conv_tc2_splitk", "gemm_tc2", "gemm_tc2_softmax", "conv_tc3"})
+# Ops whose kernels reduce with float atomics (or accumulate into a zeroed buffer): never in a deterministic plan, whose
+# recording uses the *_det ops instead (training-only ops are listed too: a deterministic plan is forward-only).
+NONDET_OPS = frozenset({"zero", "ch_stats", "gn_stats", "stem_conv_bf16", "stem_conv_s2_bf16", "conv_tc2_s2_dgrad",
+                        "gemm_tc2_major", "gemm_tc2_softmax_grad", "wgrad_tc", "wgrad_tc_bf16", "wgrad_tc_bf16_s2",
+                        "conv2d_wgrad_simt", "conv2d_dgrad_simt", "gn_bwd_sums", "gn_bwd_coef", "colsum", "embedding_bwd",
+                        "mlp_mod_ln_act_bwd", "mlp_mod_ln_act_bwd_bf16"})
+
+_LAUNCHES = {"gn_stats": 1, "attention_simt": 3, "zero": 0, "ch_stats_det": 2, "gn_stats_det": 2, "stem_conv_bf16_det": 2}

@@ -59,8 +59,16 @@ def calculate_mse(img1: torch.Tensor, img2: torch.Tensor) -> torch.Tensor:
         raise ValueError("calculate_mse: shape mismatch")
     a, b = img1.float().contiguous(), img2.float().contiguous()
     B = a.shape[0]
-    ws = torch.empty(B, dtype=torch.float64, device=a.device)
     out = torch.empty(B, dtype=torch.float32, device=a.device)
+    L = _native.lib()
+    if torch.are_deterministic_algorithms_enabled():   # per-block slots added in a fixed order: bitwise-reproducible
+        nb = L.pdae_mse_det_workspace_bytes(B, a[0].numel())
+        _native.check(min(int(nb), 0), "pdae_mse_det_workspace_bytes")
+        ws = torch.empty(max(int(nb), 8), dtype=torch.uint8, device=a.device)
+        _native.check(L.pdae_mse_per_image_det(a.data_ptr(), b.data_ptr(), B, a[0].numel(), ws.data_ptr(), ws.numel(),
+                                               out.data_ptr(), _stream(a.device)), "pdae_mse_per_image_det")
+        return out
+    ws = torch.empty(B, dtype=torch.float64, device=a.device)
     _native.check(_native.lib().pdae_mse_per_image(a.data_ptr(), b.data_ptr(), B, a[0].numel(), ws.data_ptr(), out.data_ptr(),
                                                    _stream(a.device)), "pdae_mse_per_image")
     return out
@@ -88,8 +96,17 @@ def calculate_ssim(img1: torch.Tensor, img2: torch.Tensor, window_size: int = 11
         raise ValueError("calculate_ssim: expected two [B,C,H,W] tensors of the same shape")
     a, b = img1.float().contiguous(), img2.float().contiguous()
     B, C, H, W = a.shape
-    ws = torch.empty(B, dtype=torch.float64, device=a.device)
     out = torch.empty(B, dtype=torch.float32, device=a.device)
+    L = _native.lib()
+    if torch.are_deterministic_algorithms_enabled():   # per-block slots added in a fixed order: bitwise-reproducible
+        nb = L.pdae_ssim_det_workspace_bytes(B, C, H, W)
+        _native.check(min(int(nb), 0), "pdae_ssim_det_workspace_bytes")
+        ws = torch.empty(max(int(nb), 8), dtype=torch.uint8, device=a.device)
+        _native.check(L.pdae_ssim_per_image_det(a.data_ptr(), b.data_ptr(), _window(a.device).data_ptr(), B, C, H, W,
+                                                ws.data_ptr(), ws.numel(), out.data_ptr(), _stream(a.device)),
+                      "pdae_ssim_per_image_det")
+        return out
+    ws = torch.empty(B, dtype=torch.float64, device=a.device)
     _native.check(_native.lib().pdae_ssim_per_image(a.data_ptr(), b.data_ptr(), _window(a.device).data_ptr(), B, C, H, W,
                                                     ws.data_ptr(), out.data_ptr(), _stream(a.device)), "pdae_ssim_per_image")
     return out

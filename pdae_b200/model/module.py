@@ -139,11 +139,13 @@ class PlannedModule(nn.Module):
 
     def _get_plan(self, key, builder):
         prec = self.precision or get_default_precision()
-        key = (key, prec)
+        # torch.use_deterministic_algorithms: the deterministic plan (engine.py), cached beside the default one
+        det = torch.are_deterministic_algorithms_enabled()
+        key = (key, prec, det)
         plans = self._plans()
         ent = plans.get(key)
         if ent is None or ent[0].stale():
-            plan = Plan(self._device(), prec)
+            plan = Plan(self._device(), prec, deterministic=det)
             io = builder(plan)
             plan.finalize()
             ent = (plan, io)

@@ -11,7 +11,7 @@ from typing import List
 import torch
 import torch.nn as nn
 
-from ....engine import _STREAM, Plan, RESAMPLE_NONE
+from ....engine import Plan, RESAMPLE_NONE
 from ...module import AttentionBlock, PlannedModule, Slots, Src, normalization
 
 
@@ -85,14 +85,13 @@ class ConvStackEncoder(PlannedModule):
     def _emit_stem(self, P: Plan, m: nn.Conv2d, x_in, B: int, H: int, W: int) -> Src:
         Co = m.weight.shape[0]
         Ho, Wo = H // 2, W // 2
-        if P.stream_bf16 and Co % 8 == 0 and Co <= 256 and W % 8 == 0:
+        if P.stream_bf16 and Co % 8 == 0 and Co <= 256 and W % 8 == 0 and P.stem_det_fits(3, Co):
             # bf16 stream from the first layer: the stride-2 stem writes bf16 NHWC and the first GroupNorm's statistics
             wt = m.weight
             wp = P.pack((id(wt), "stem"), [wt], lambda: wt.detach().reshape(Co, 3, 9).permute(2, 1, 0).float())   # [9][Cin][Cout]
             out = P.new((B, Ho, Wo, Co), torch.bfloat16, "enc_stem")
-            st = P.new_stats(B, Co)
-            P.call("stem_conv_s2_bf16", x_in, wp, P.param(m.bias), out, st, B, H, W, 3, Co, _STREAM,
-                   flops=2.0 * B * Ho * Wo * Co * 3 * 9)
+            st = P.stem_conv_bf16(x_in, wp, m.bias, out, B=B, H=H, W=W, Cin=3, Cout=Co, stride=2,
+                                  flops=2.0 * B * Ho * Wo * Co * 3 * 9)
             return Src(out, Co, B, Ho, Wo, s1=st)
         out = P.new((B, Ho, Wo, Co), torch.float32, "enc_h")
         P.conv(x_in, m.weight, m.bias, out, B=B, H=H, W=W, Cin=3, Cout=Co, k=3, stride=2, pad=1, in_nchw=True)

@@ -116,13 +116,12 @@ def emit_stem(P: Plan, stem: nn.Module, x_in: Buf, B: int, H: int, W: int, Cin: 
     of them); otherwise the generic CUDA-core conv (+ a statistics pass in fused-statistics mode)."""
     c0 = stem.weight.shape[0]
     if (P.fused_stats and P.stream_bf16 and Cin <= 4 and c0 % 8 == 0 and c0 <= 256 and stem.kernel_size[0] == 3
-            and W % 4 == 0):
+            and W % 4 == 0 and P.stem_det_fits(Cin, c0)):
         wt = stem.weight
         wp = P.pack((id(wt), "stem"), [wt], lambda: wt.detach().reshape(c0, Cin, 9).permute(2, 1, 0).float())   # [9][Cin][Cout]
         h0 = P.new((B, H, W, c0), torch.bfloat16, "stem")
-        st0 = P.new_stats(B, c0)
-        P.call("stem_conv_bf16", x_in, wp, P.param(stem.bias), h0, st0, B, H, W, Cin, c0, _STREAM,
-               flops=2.0 * B * H * W * c0 * Cin * 9)
+        st0 = P.stem_conv_bf16(x_in, wp, stem.bias, h0, B=B, H=H, W=W, Cin=Cin, Cout=c0, stride=1,
+                               flops=2.0 * B * H * W * c0 * Cin * 9)
         return Src(h0, c0, B, H, W, s1=st0)
     h0 = P.new((B, H, W, c0), torch.float32, "stem")
     P.conv(x_in, stem.weight, stem.bias, h0, B=B, H=H, W=W, Cin=Cin, Cout=c0, k=3, in_nchw=True)

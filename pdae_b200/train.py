@@ -31,6 +31,7 @@ from __future__ import annotations
 
 import ctypes
 import math
+import warnings
 from typing import Callable, Dict, List, Optional, Tuple
 
 import numpy as np
@@ -374,8 +375,16 @@ class _Generation:
     backward) instead of returning silently wrong gradients."""
     _gen = 0
     _consumed = -1
+    _det_warned = False
 
     def _stamp(self) -> int:
+        if torch.are_deterministic_algorithms_enabled() and not self._det_warned:
+            # the training plans keep their atomic reductions (weight gradients, GroupNorm backward): say so once, do not raise,
+            # so that a training run with the switch on keeps working
+            self._det_warned = True
+            warnings.warn(f"pdae_b200 {type(self).__name__}: the training forward/backward has no deterministic implementation "
+                          "yet; torch.use_deterministic_algorithms covers the pdae_b200 forward-only and sampling paths only",
+                          UserWarning, stacklevel=3)
         self._gen += 1
         return self._gen
 
