@@ -213,6 +213,37 @@ int pdae_dsilu_mul(const float* g, const float* x, float* out, int64_t n, pdae_s
 int pdae_add_inplace(float* a, const float* b, int64_t n, pdae_stream_t stream);
 /* inverted dropout (nn.Dropout in out_layers, module.py:259): a *= mask * scale with a caller-drawn 0/1 mask.            */
 int pdae_mul_mask(float* a, const float* mask, float scale, int64_t n, pdae_stream_t stream);
+/* Deterministic forms of the backward (torch.use_deterministic_algorithms in training): no float atomics; every partial result
+ * is stored in its own slot of the caller-owned workspace (no initialisation needed; *_workspace_bytes bytes, 0 = none needed,
+ * negative = bad arguments) and the slots are summed in a fixed order.  Split and chunk counts follow the shapes only.  The
+ * outputs are WRITTEN, not added to: dw, out, S, dgamma / dbeta and the embedding gradient need no zeroing.
+ *  wgrad_simt_det: pixel chunk z -> slot z of [chunks][k*k*Cin][Cout], summed in chunk order (one chunk: straight into dw).
+ *  dgrad_simt_det: as pdae_conv2d_dgrad_simt; the wide-Linear split-K form (H = W = 1, Cout >= 1024) slots [Cout/64][B][Cin].
+ *  colsum_det:     row chunk -> slot of [chunks][N].
+ *  gn_bwd_sums_det: per-CTA (sum du, sum du*x) slots [B][P][C][2] reduced in P order into S [B][C][2] (same layout).
+ *  gn_bwd_coef_det: group sums added in channel order; dgamma / dbeta through per-image slots [2][B][C] summed over b in order
+ *                   (workspace only when dgamma or dbeta is given; C % 32 == 0, C <= 2048).
+ *  embedding_bwd_det: dw[rows][E] = for every row r, the sum over b (in order) of d_emb[b] with idx[b] == r.                  */
+int64_t pdae_conv2d_wgrad_simt_det_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int stride, int pad);
+int pdae_conv2d_wgrad_simt_det(const float* x, int in_nchw, int a_silu, const float* dy, float* dw_tcico, int B, int H, int W,
+                               int Cin, int Cout, int ksize, int stride, int pad, float* workspace, int64_t workspace_bytes,
+                               pdae_stream_t stream);
+int64_t pdae_conv2d_dgrad_simt_det_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int stride, int pad,
+                                                   int accumulate);
+int pdae_conv2d_dgrad_simt_det(const float* dy, const float* w_tco, float* dx, int B, int H, int W, int Cin, int Cout, int ksize,
+                               int stride, int pad, int accumulate, float* workspace, int64_t workspace_bytes, pdae_stream_t stream);
+int64_t pdae_colsum_det_workspace_bytes(int64_t M, int N);
+int pdae_colsum_det(const float* dy, int64_t M, int N, float* out, float* workspace, int64_t workspace_bytes, pdae_stream_t stream);
+int64_t pdae_gn_bwd_sums_det_workspace_bytes(int B, int H, int W, int C);
+int pdae_gn_bwd_sums_det(const float* src1, int C1, const float* src2, int C2, const float* ab, const float* dy, int silu,
+                         int resample, int B, int H, int W, float* S, float* workspace, int64_t workspace_bytes,
+                         pdae_stream_t stream);
+int64_t pdae_gn_bwd_coef_det_workspace_bytes(int B, int C);
+int pdae_gn_bwd_coef_det(const float* S, const double* sums, const float* gamma, const float* beta, const float* emb, int emb_ld,
+                         const float* embz, int embz_ld, int B, int C, int HW, float eps, float* kk, float* dgamma, float* dbeta,
+                         float* demb, int demb_ld, float* dembz, int dembz_ld, float* workspace, int64_t workspace_bytes,
+                         pdae_stream_t stream);
+int pdae_embedding_bwd_det(const float* d_emb, const int64_t* idx, float* dw, int B, int E, int rows, pdae_stream_t stream);
 /* MLPLNAct backward (model/mlp_skip_net.py:123-141; latent DPM training, gaussian_diffusion.py:373-398): given
  * dy = grad of y = SiLU(LN(h*(1+cond))) (read with leading dimension dy_ld) -> dh, dcond [B][N] and the LayerNorm
  * parameter gradients accumulated into d_ln_w / d_ln_b (zero them first).  ln_w == NULL: no LayerNorm.                  */
@@ -277,6 +308,13 @@ int pdae_wgrad_tc_create_bf16(pdae_wgrad_tc_plan** plan, const void* act_bf16, c
  * dy: [B][H/2][W/2][Cout], H and W even, channels as pdae_conv_s2_tc_supported.  Same zeroing contract and run / destroy. */
 int pdae_wgrad_tc_create_bf16_s2(pdae_wgrad_tc_plan** plan, const void* act_bf16, const void* dy_bf16, float* dw, int B, int H,
                                  int W, int Cin, int Cout);
+/* Deterministic plans: switch any wgrad_tc plan to its DET kernel (no float atomics).  Work unit = (output tile group, pixel
+ * split); each split stores its partial dw into its own slot [splits][k*k][Cin][Cout] of the caller-owned workspace and the run
+ * adds the slots in split order into dw, which then needs no zeroing.  The split count follows the shape only (about one wave
+ * of units on a 132-SM H100); with one split (workspace 0) the kernel stores straight into dw.  Call once, after create and
+ * before the first run; workspace: pdae_wgrad_tc_det_workspace_bytes(plan) bytes.                                          */
+int64_t pdae_wgrad_tc_det_workspace_bytes(const pdae_wgrad_tc_plan* plan);
+int pdae_wgrad_tc_set_deterministic(pdae_wgrad_tc_plan* plan, float* workspace, int64_t workspace_bytes);
 int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* plan, pdae_stream_t stream);
 void pdae_wgrad_tc_destroy(pdae_wgrad_tc_plan* plan);
 

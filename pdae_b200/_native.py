@@ -92,6 +92,20 @@ _SIGS = {
                                  c_int, _P]),
     "pdae_gn_bwd_apply": (c_int, [_P, c_int, _P, c_int, _P, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, c_int, _P, _P, _P]),
     "pdae_embedding_bwd": (c_int, [_P, _P, _P, c_int, c_int, _P]),
+    "pdae_conv2d_wgrad_simt_det_workspace_bytes": (c_int64, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_conv2d_wgrad_simt_det": (c_int, [_P, c_int, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P,
+                                           c_int64, _P]),
+    "pdae_conv2d_dgrad_simt_det_workspace_bytes": (c_int64, [c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_conv2d_dgrad_simt_det": (c_int, [_P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, c_int, _P, c_int64,
+                                           _P]),
+    "pdae_colsum_det_workspace_bytes": (c_int64, [c_int64, c_int]),
+    "pdae_colsum_det": (c_int, [_P, c_int64, c_int, _P, _P, c_int64, _P]),
+    "pdae_gn_bwd_sums_det_workspace_bytes": (c_int64, [c_int, c_int, c_int, c_int]),
+    "pdae_gn_bwd_sums_det": (c_int, [_P, c_int, _P, c_int, _P, _P, c_int, c_int, c_int, c_int, c_int, _P, _P, c_int64, _P]),
+    "pdae_gn_bwd_coef_det_workspace_bytes": (c_int64, [c_int, c_int]),
+    "pdae_gn_bwd_coef_det": (c_int, [_P, _P, _P, _P, _P, c_int, _P, c_int, c_int, c_int, c_int, c_float, _P, _P, _P, _P, c_int, _P,
+                                     c_int, _P, c_int64, _P]),
+    "pdae_embedding_bwd_det": (c_int, [_P, _P, _P, c_int, c_int, c_int, _P]),
     "pdae_softmax_bwd": (c_int, [_P, _P, c_int64, c_int, c_float, _P]),
     "pdae_dsilu_mul": (c_int, [_P, _P, _P, c_int64, _P]),
     "pdae_add_inplace": (c_int, [_P, _P, c_int64, _P]),
@@ -133,6 +147,8 @@ _SIGS = {
     "pdae_wgrad_tc_create": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_create_bf16": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int, c_int]),
     "pdae_wgrad_tc_create_bf16_s2": (c_int, [POINTER(c_void_p), _P, _P, _P, c_int, c_int, c_int, c_int, c_int]),
+    "pdae_wgrad_tc_det_workspace_bytes": (c_int64, [_P]),
+    "pdae_wgrad_tc_set_deterministic": (c_int, [_P, _P, c_int64]),
     "pdae_wgrad_tc_run": (c_int, [_P, _P]),
     "pdae_wgrad_tc_destroy": (None, [_P]),
     "pdae_softmax_bf16": (c_int, [_P, _P, c_int64, c_int, c_float, _P]),

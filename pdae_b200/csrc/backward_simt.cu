@@ -100,6 +100,8 @@ struct WgradArgs {
 };
 
 // dw[tap*Cin+ci][co] += sum_{pixels} f(x[b, oy*s-p+ky, ox*s-p+kx, ci]) * dy[pixel][co]    (split over pixel chunks, atomics)
+// DET: pixel chunk z stores its partial into slot z of p.dw ([chunks][MK][Cout]); the slots are summed in order afterwards
+template <bool DET>
 __global__ void __launch_bounds__(256) conv_wgrad_kernel(WgradArgs p) {
   __shared__ __align__(16) float As[DBK][DBM + 4];   // [pixel][row of dw]
   __shared__ __align__(16) float Bs[DBK][DBN];       // [pixel][co]
@@ -171,23 +173,29 @@ __global__ void __launch_bounds__(256) conv_wgrad_kernel(WgradArgs p) {
     if (r >= p.MK) continue;
     for (int j = 0; j < 4; ++j) {
       const int n = n0 + tx * 4 + j;
-      if (n < p.Cout) atomicAdd(p.dw + (long long)r * p.Cout + n, acc[i][j]);
+      if (n >= p.Cout) continue;
+      if constexpr (DET) p.dw[((long long)blockIdx.z * p.MK + r) * p.Cout + n] = acc[i][j];
+      else atomicAdd(p.dw + (long long)r * p.Cout + n, acc[i][j]);
     }
   }
 }
 
-// out[n] += sum_m dy[m][n]
+// out[n] += sum_m dy[m][n]   (DET: row chunk x stores its sums into slot x of out, [chunks][N])
+template <bool DET>
 __global__ void colsum_kernel(const float* __restrict__ dy, long long M, int N, float* __restrict__ out, int rows_per_cta) {
   const long long m0 = (long long)blockIdx.x * rows_per_cta, m1 = min(M, m0 + rows_per_cta);
   for (int n = threadIdx.x; n < N; n += blockDim.x) {
     float s = 0.f;
     for (long long m = m0; m < m1; ++m) s += dy[m * N + n];
-    atomicAdd(out + n, s);
+    if constexpr (DET) out[(long long)blockIdx.x * N + n] = s;
+    else atomicAdd(out + n, s);
   }
 }
 
 // N % 4 == 0: a warp reads 32 float4 columns (512 contiguous bytes) of one row, the 8 warps of a CTA take interleaved rows
 // (four independent loads in flight per thread), partial sums meet in shared memory, one fp32 reduction per column and CTA
+// (DET: one plain store per column into the CTA's slot of out, [chunks][N])
+template <bool DET>
 __global__ void __launch_bounds__(256) colsum_v4_kernel(const float* __restrict__ dy, long long M, int N, float* __restrict__ out,
                                                         int rows_per_cta) {
   __shared__ float4 part[8][32];
@@ -217,8 +225,13 @@ __global__ void __launch_bounds__(256) colsum_v4_kernel(const float* __restrict_
         const float4 t = part[i][lane];
         s.x += t.x; s.y += t.y; s.z += t.z; s.w += t.w;
       }
-      float* o = out + 4 * cv;
-      atomicAdd(o, s.x); atomicAdd(o + 1, s.y); atomicAdd(o + 2, s.z); atomicAdd(o + 3, s.w);
+      if constexpr (DET) {
+        float* o = out + (long long)blockIdx.x * N + 4 * cv;
+        o[0] = s.x; o[1] = s.y; o[2] = s.z; o[3] = s.w;
+      } else {
+        float* o = out + 4 * cv;
+        atomicAdd(o, s.x); atomicAdd(o + 1, s.y); atomicAdd(o + 2, s.z); atomicAdd(o + 3, s.w);
+      }
     }
     __syncthreads();
   }
@@ -251,19 +264,23 @@ __device__ __forceinline__ float dsilu(float u) {
   return s * (1.0f + u * (1.0f - s));
 }
 
-template <int RS>
+// DET: the pixel rows of a CTA keep their own shared sums ([R][2][C], no shared atomics), added in row order; the CTA stores
+// them into its slot S[b][blockIdx.x][C][2], and stat_parts_reduce sums the slots in order (the ch_parts_kernel pattern).
+template <int RS, bool DET>
 __global__ void __launch_bounds__(256) gn_bwd_sums_kernel(const float* __restrict__ s1, int C1, const float* __restrict__ s2,
                                                           int C2, const float* __restrict__ ab, const float* __restrict__ dy,
                                                           int silu, int H, int W, float* __restrict__ S, int ppc) {
-  extern __shared__ float sh[];  // [2][C]
+  extern __shared__ float sh[];  // [2][C]; DET: [R][2][C]
   const int C = C1 + C2, L = C >> 2;
   const int Lb = L < 256 ? L : 256, R = 256 / Lb;
   const int tid = threadIdx.x, lane = tid % Lb, row = tid / Lb;
   const int b = blockIdx.y;
   const int HW = H * W;
   const int p0 = blockIdx.x * ppc, p1 = min(HW, p0 + ppc);     // ppc pixels per CTA (host: enough CTAs to fill the SMs)
-  for (int i = tid; i < 2 * C; i += 256) sh[i] = 0.f;
-  __syncthreads();
+  if (!DET) {
+    for (int i = tid; i < 2 * C; i += 256) sh[i] = 0.f;
+    __syncthreads();
+  }
   if (row < R) {
     for (int cq = lane; cq < L; cq += Lb) {
       const int c = cq * 4;
@@ -284,30 +301,50 @@ __global__ void __launch_bounds__(256) gn_bwd_sums_kernel(const float* __restric
         t1.x += g.x; t1.y += g.y; t1.z += g.z; t1.w += g.w;
         t2.x = fmaf(g.x, xv.x, t2.x); t2.y = fmaf(g.y, xv.y, t2.y); t2.z = fmaf(g.z, xv.z, t2.z); t2.w = fmaf(g.w, xv.w, t2.w);
       }
-      atomicAdd(&sh[c + 0], t1.x); atomicAdd(&sh[c + 1], t1.y); atomicAdd(&sh[c + 2], t1.z); atomicAdd(&sh[c + 3], t1.w);
-      atomicAdd(&sh[C + c + 0], t2.x); atomicAdd(&sh[C + c + 1], t2.y); atomicAdd(&sh[C + c + 2], t2.z); atomicAdd(&sh[C + c + 3], t2.w);
+      if constexpr (DET) {
+        *reinterpret_cast<float4*>(sh + (size_t)row * 2 * C + c) = t1;
+        *reinterpret_cast<float4*>(sh + (size_t)row * 2 * C + C + c) = t2;
+      } else {
+        atomicAdd(&sh[c + 0], t1.x); atomicAdd(&sh[c + 1], t1.y); atomicAdd(&sh[c + 2], t1.z); atomicAdd(&sh[c + 3], t1.w);
+        atomicAdd(&sh[C + c + 0], t2.x); atomicAdd(&sh[C + c + 1], t2.y); atomicAdd(&sh[C + c + 2], t2.z); atomicAdd(&sh[C + c + 3], t2.w);
+      }
     }
   }
   __syncthreads();
-  for (int c = tid; c < C; c += 256) {
-    atomicAdd(&S[((long long)b * C + c) * 2 + 0], sh[c]);
-    atomicAdd(&S[((long long)b * C + c) * 2 + 1], sh[C + c]);
+  if constexpr (DET) {
+    for (int c = tid; c < C; c += 256) {
+      float a = 0.f, q = 0.f;
+      for (int r = 0; r < R; ++r) {
+        a += sh[(size_t)r * 2 * C + c];
+        q += sh[(size_t)r * 2 * C + C + c];
+      }
+      *reinterpret_cast<float2*>(S + (((long long)b * gridDim.x + blockIdx.x) * C + c) * 2) = make_float2(a, q);
+    }
+  } else {
+    for (int c = tid; c < C; c += 256) {
+      atomicAdd(&S[((long long)b * C + c) * 2 + 0], sh[c]);
+      atomicAdd(&S[((long long)b * C + c) * 2 + 1], sh[C + c]);
+    }
   }
 }
 
 // pass 2 (tiny): from S1,S2, the forward statistics and the modulation rows produce
 //   k[b][0][c] = gt*rstd (dx = k*du - (cA + x*cB) ...), per-group cA, cB folded per channel into kk[b][1..2][c],
 //   gradients of gamma/beta (atomics over b) and of the (scale|shift) rows of emb / embz.
+// DET: the per-channel terms of the group sums sit in shared memory ([2][C] doubles) and one thread per group adds them in
+// channel order; dgamma / dbeta point at per-image slots [B][C], which gn_param_reduce_kernel sums over b in order.
+template <bool DET>
 __global__ void gn_bwd_coef_kernel(const float* __restrict__ S, const double* __restrict__ sums, const float* __restrict__ gamma,
                                    const float* __restrict__ beta, const float* __restrict__ emb, int emb_ld,
                                    const float* __restrict__ embz, int embz_ld, int C, int HW, float eps,
                                    float* __restrict__ kk, float* __restrict__ dgamma, float* __restrict__ dbeta,
                                    float* __restrict__ demb, int demb_ld, float* __restrict__ dembz, int dembz_ld) {
   __shared__ double gA[32], gB[32];
+  extern __shared__ double terms[];   // DET: [2][C]
   const int b = blockIdx.x;
   const int cpg = C / 32;
   const double n = (double)HW * cpg;
-  if (threadIdx.x < 32) { gA[threadIdx.x] = 0.0; gB[threadIdx.x] = 0.0; }
+  if (!DET && threadIdx.x < 32) { gA[threadIdx.x] = 0.0; gB[threadIdx.x] = 0.0; }
   __syncthreads();
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const int g = c / cpg;
@@ -322,11 +359,18 @@ __global__ void gn_bwd_coef_kernel(const float* __restrict__ S, const double* __
     const double S1 = S[((long long)b * C + c) * 2], S2 = S[((long long)b * C + c) * 2 + 1];
     const double dbt = S1;                                   // d beta~  = sum du
     const double dgt = rstd * (S2 - mean * S1);              // d gamma~ = sum du * xhat
-    atomicAdd(&gA[g], (double)gt * dbt);
-    atomicAdd(&gB[g], (double)gt * dgt);
     // parameter / modulation gradients
-    if (dgamma) atomicAdd(dgamma + c, (float)(dgt * s * zs));
-    if (dbeta) atomicAdd(dbeta + c, (float)(dbt * s * zs));
+    if constexpr (DET) {
+      terms[c] = (double)gt * dbt;
+      terms[C + c] = (double)gt * dgt;
+      if (dgamma) dgamma[(long long)b * C + c] = (float)(dgt * s * zs);
+      if (dbeta) dbeta[(long long)b * C + c] = (float)(dbt * s * zs);
+    } else {
+      atomicAdd(&gA[g], (double)gt * dbt);
+      atomicAdd(&gB[g], (double)gt * dgt);
+      if (dgamma) atomicAdd(dgamma + c, (float)(dgt * s * zs));
+      if (dbeta) atomicAdd(dbeta + c, (float)(dbt * s * zs));
+    }
     if (demb) {
       demb[(long long)b * demb_ld + c] = (float)((dgt * gamma[c] + dbt * beta[c]) * zs);
       demb[(long long)b * demb_ld + C + c] = (float)(dbt * zs);
@@ -337,6 +381,15 @@ __global__ void gn_bwd_coef_kernel(const float* __restrict__ S, const double* __
     }
   }
   __syncthreads();
+  if constexpr (DET) {
+    if (threadIdx.x < 32) {
+      double a = 0.0, q = 0.0;
+      for (int c = threadIdx.x * cpg; c < (threadIdx.x + 1) * cpg; ++c) { a += terms[c]; q += terms[C + c]; }
+      gA[threadIdx.x] = a;
+      gB[threadIdx.x] = q;
+    }
+    __syncthreads();
+  }
   for (int c = threadIdx.x; c < C; c += blockDim.x) {
     const int g = c / cpg;
     const double mean = sums[((long long)b * 32 + g) * 2] / n;
@@ -397,6 +450,37 @@ __global__ void __launch_bounds__(256) gn_bwd_apply_kernel(const float* __restri
   }
 }
 
+// dgamma[c] = sum over b in order of part[b][c] (and dbeta from part + B*C): the deterministic gn_bwd_coef's second pass
+__global__ void gn_param_reduce_kernel(const float* __restrict__ part, int B, int C, float* __restrict__ dgamma,
+                                       float* __restrict__ dbeta) {
+  const int c = blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= C) return;
+  if (dgamma) {
+    float a = 0.f;
+    for (int b = 0; b < B; ++b) a += part[(long long)b * C + c];
+    dgamma[c] = a;
+  }
+  if (dbeta) {
+    float a = 0.f;
+    for (int b = 0; b < B; ++b) a += part[((long long)B + b) * C + c];
+    dbeta[c] = a;
+  }
+}
+
+// out[i] = sum over s = 0, 1, ..., S-1 in order of part[s][i]: the ordered reduction of per-split slots
+__global__ void __launch_bounds__(256) slot_sum_kernel(const float* __restrict__ part, int S, long long n, float* __restrict__ out) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  float a = part[i];
+  for (int k = 1; k < S; ++k) a += part[(long long)k * n + i];
+  out[i] = a;
+}
+
+cudaError_t launch_slot_sum(const float* part, int S, long long n, float* out, cudaStream_t s) {
+  slot_sum_kernel<<<cdiv(n, 256), 256, 0, s>>>(part, S, n, out);
+  return cudaPeekAtLastError();
+}
+
 // dW[idx[b]][:] += d_emb[b][:]   (nn.Embedding backward, unet.py:190-192)
 __global__ void embedding_bwd_kernel(const float* __restrict__ d_emb, const int64_t* __restrict__ idx, float* __restrict__ dw,
                                      int B, int E) {
@@ -404,6 +488,18 @@ __global__ void embedding_bwd_kernel(const float* __restrict__ d_emb, const int6
   if (i >= B * E) return;
   const int b = i / E, j = i % E;
   atomicAdd(dw + idx[b] * E + j, d_emb[i]);
+}
+
+// deterministic form: dW[r][j] = sum over b in order of d_emb[b][j] where idx[b] == r, for every row r (rows without a label get 0)
+__global__ void embedding_bwd_det_kernel(const float* __restrict__ d_emb, const int64_t* __restrict__ idx, float* __restrict__ dw,
+                                         int B, int E, int rows) {
+  const long long i = (long long)blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= (long long)rows * E) return;
+  const int r = (int)(i / E), j = (int)(i % E);
+  float a = 0.f;
+  for (int b = 0; b < B; ++b)
+    if (idx[b] == r) a += d_emb[(long long)b * E + j];
+  dw[i] = a;
 }
 
 // dS = alpha * P * (dP - rowsum(dP * P)), in place on dP  (softmax backward with the ch^-1/2 scale folded in)
@@ -574,6 +670,8 @@ __global__ void mul_mask_cols_kernel(float* __restrict__ a, int ld, const float*
 
 // dgrad of a wide Linear (H = W = 1, k = 1, Cout = N large): dx[b][e] = sum_n dy[b][n] * w[n][e].  The generic kernel gives one
 // thread a serial reduction over all N; here each CTA owns a 64-row chunk of w (split-K) and adds its partial sums.
+// DET: chunk x stores its partial sums into slot x of dx ([chunks][B][E]), summed in order by slot_sum_kernel.
+template <bool DET>
 __global__ void __launch_bounds__(256) linear_dgrad_splitk_kernel(const float* __restrict__ dy, const float* __restrict__ w,
                                                                   float* __restrict__ dx, int B, int N, int E) {
   __shared__ float ds[32][65];
@@ -597,7 +695,10 @@ __global__ void __launch_bounds__(256) linear_dgrad_splitk_kernel(const float* _
       }
 #pragma unroll
       for (int i = 0; i < 8; ++i)
-        if (b0 + bb + i < B) atomicAdd(dx + (long long)(b0 + bb + i) * E + e, acc[i]);
+        if (b0 + bb + i < B) {
+          if constexpr (DET) dx[((long long)blockIdx.x * B + b0 + bb + i) * E + e] = acc[i];
+          else atomicAdd(dx + (long long)(b0 + bb + i) * E + e, acc[i]);
+        }
     }
   }
 }
@@ -650,7 +751,7 @@ extern "C" int pdae_conv2d_dgrad_simt(const float* dy, const float* w_tco, float
   PDAE_REQUIRE(dy && w_tco && dx, "conv2d_dgrad: null pointer");
   if (H == 1 && W == 1 && ksize == 1 && stride == 1 && pad == 0 && Cout >= 1024 && !accumulate) {   // wide Linear: split-K
     PDAE_CUDA(cudaMemsetAsync(dx, 0, (size_t)B * Cin * sizeof(float), (cudaStream_t)stream));
-    linear_dgrad_splitk_kernel<<<dim3(cdiv(Cout, 64), cdiv(Cin, 256)), 256, 0, (cudaStream_t)stream>>>(dy, w_tco, dx, B, Cout, Cin);
+    linear_dgrad_splitk_kernel<false><<<dim3(cdiv(Cout, 64), cdiv(Cin, 256)), 256, 0, (cudaStream_t)stream>>>(dy, w_tco, dx, B, Cout, Cin);
     PDAE_LAUNCH_CHECK("linear_dgrad_splitk_kernel");
     return PDAE_OK;
   }
@@ -692,7 +793,7 @@ extern "C" int pdae_conv2d_wgrad_simt(const float* x, int in_nchw, int a_silu, c
   p.chunk = (int)(((p.P + splits - 1) / splits + DBK - 1) / DBK * DBK);
   const int gz = (int)((p.P + p.chunk - 1) / p.chunk);
   dim3 grid(gx, gy, gz);
-  conv_wgrad_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(p);
+  conv_wgrad_kernel<false><<<grid, 256, 0, (cudaStream_t)stream>>>(p);
   PDAE_LAUNCH_CHECK("conv_wgrad_kernel");
   return PDAE_OK;
 }
@@ -702,12 +803,12 @@ extern "C" int pdae_colsum(const float* dy, int64_t M, int N, float* out, pdae_s
   if (N % 4 == 0 && !((uintptr_t)dy & 15)) {
     long long rows = (M / 592 + 7) / 8 * 8;      // about four CTAs per SM, eight-row granules
     rows = rows < 32 ? 32 : (rows > 512 ? 512 : rows);
-    colsum_v4_kernel<<<(unsigned)cdiv(M, rows), 256, 0, (cudaStream_t)stream>>>(dy, M, N, out, (int)rows);
+    colsum_v4_kernel<false><<<(unsigned)cdiv(M, rows), 256, 0, (cudaStream_t)stream>>>(dy, M, N, out, (int)rows);
     PDAE_LAUNCH_CHECK("colsum_v4_kernel");
     return PDAE_OK;
   }
   const int rows = 256;
-  colsum_kernel<<<cdiv(M, rows), N < 256 ? (N < 32 ? 32 : N) : 256, 0, (cudaStream_t)stream>>>(dy, M, N, out, rows);
+  colsum_kernel<false><<<cdiv(M, rows), N < 256 ? (N < 32 ? 32 : N) : 256, 0, (cudaStream_t)stream>>>(dy, M, N, out, rows);
   PDAE_LAUNCH_CHECK("colsum_kernel");
   return PDAE_OK;
 }
@@ -726,9 +827,9 @@ extern "C" int pdae_gn_bwd_sums(const float* src1, int C1, const float* src2, in
   while (ppc > 8 && (long long)B * cdiv((long long)H * W, ppc) < 592) ppc >>= 1;
   dim3 grid(cdiv((long long)H * W, ppc), B);
   const size_t sm = 2 * C * sizeof(float);
-  if (resample == PDAE_RESAMPLE_NONE) gn_bwd_sums_kernel<PDAE_RESAMPLE_NONE><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, S, ppc);
-  else if (resample == PDAE_RESAMPLE_UP2) gn_bwd_sums_kernel<PDAE_RESAMPLE_UP2><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, S, ppc);
-  else gn_bwd_sums_kernel<PDAE_RESAMPLE_DOWN2><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, S, ppc);
+  if (resample == PDAE_RESAMPLE_NONE) gn_bwd_sums_kernel<PDAE_RESAMPLE_NONE, false><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, S, ppc);
+  else if (resample == PDAE_RESAMPLE_UP2) gn_bwd_sums_kernel<PDAE_RESAMPLE_UP2, false><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, S, ppc);
+  else gn_bwd_sums_kernel<PDAE_RESAMPLE_DOWN2, false><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, S, ppc);
   PDAE_LAUNCH_CHECK("gn_bwd_sums_kernel");
   return PDAE_OK;
 }
@@ -738,7 +839,7 @@ extern "C" int pdae_gn_bwd_coef(const float* S, const double* sums, const float*
                                 float* dgamma, float* dbeta, float* demb, int demb_ld, float* dembz, int dembz_ld,
                                 pdae_stream_t stream) {
   PDAE_REQUIRE(S && sums && gamma && beta && kk, "gn_bwd_coef: null pointer");
-  gn_bwd_coef_kernel<<<B, C < 1024 ? (C < 32 ? 32 : C) : 1024, 0, (cudaStream_t)stream>>>(
+  gn_bwd_coef_kernel<false><<<B, C < 1024 ? (C < 32 ? 32 : C) : 1024, 0, (cudaStream_t)stream>>>(
       S, sums, gamma, beta, emb, emb_ld, embz, embz_ld, C, HW, eps, kk, dgamma, dbeta, demb, demb_ld, dembz, dembz_ld);
   PDAE_LAUNCH_CHECK("gn_bwd_coef_kernel");
   return PDAE_OK;
@@ -837,5 +938,200 @@ extern "C" int pdae_mul_mask_cols(float* a, int ld, const float* mask, float sca
   PDAE_REQUIRE(a && mask && B > 0 && N > 0 && ld >= N, "mul_mask_cols: bad args");
   mul_mask_cols_kernel<<<cdiv((long long)B * N, 256), 256, 0, (cudaStream_t)stream>>>(a, ld, mask, scale, B, N);
   PDAE_LAUNCH_CHECK("mul_mask_cols_kernel");
+  return PDAE_OK;
+}
+
+// ---- deterministic forms (torch.use_deterministic_algorithms): no float atomics -------------------------------------------
+// Every partial result has its own slot in a caller-owned workspace (no initialisation needed) and the slots are summed in a
+// fixed order.  Split and chunk counts follow the shapes only, never the GPU.  Arguments and the workspace size are checked
+// before any launch; the outputs are written, not added to, so they need no zeroing.
+namespace pdae {
+constexpr int DET_WGRAD_CTAS = 132 * 4;   // conv_wgrad_kernel: about four CTAs per SM of a 132-SM H100, a constant
+
+static void wgrad_simt_args(WgradArgs& p, int B, int H, int W, int Cin, int Cout, int ksize, int stride, int pad) {
+  p.B = B; p.H = H; p.W = W; p.Cin = Cin; p.Cout = Cout; p.ksize = ksize; p.stride = stride; p.pad = pad;
+  p.Ho = (H + 2 * pad - ksize) / stride + 1; p.Wo = (W + 2 * pad - ksize) / stride + 1;
+  p.P = (long long)B * p.Ho * p.Wo; p.MK = ksize * ksize * Cin;
+  const long long tiles = (long long)cdiv(p.MK, DBM) * cdiv(Cout, DBN);
+  long long splits = (DET_WGRAD_CTAS + tiles - 1) / tiles, maxs = (p.P + 255) / 256;
+  if (splits > maxs) splits = maxs;
+  if (splits < 1) splits = 1;
+  p.chunk = (int)(((p.P + splits - 1) / splits + DBK - 1) / DBK * DBK);
+}
+static bool wgrad_simt_shape_ok(int B, int H, int W, int Cin, int Cout, int ksize, int stride, int pad) {
+  return B > 0 && H > 0 && W > 0 && Cin > 0 && Cout > 0 && ksize > 0 && stride > 0 && pad >= 0 && H + 2 * pad >= ksize &&
+         W + 2 * pad >= ksize;
+}
+static long long colsum_det_rows(long long M) {   // pdae_colsum's row chunk, used by both deterministic paths
+  long long rows = (M / 592 + 7) / 8 * 8;
+  return rows < 32 ? 32 : (rows > 512 ? 512 : rows);
+}
+static int gn_bwd_ppc(int B, int HW) {            // pdae_gn_bwd_sums' pixels per CTA (a function of B and HW)
+  int ppc = 256;
+  while (ppc > 8 && (long long)B * cdiv((long long)HW, ppc) < 592) ppc >>= 1;
+  return ppc;
+}
+static bool dgrad_wide_linear(int H, int W, int ksize, int stride, int pad, int Cout, int accumulate) {
+  return H == 1 && W == 1 && ksize == 1 && stride == 1 && pad == 0 && Cout >= 1024 && !accumulate;
+}
+}  // namespace pdae
+
+#define PDAE_DET_WS(fn, need, ws, ws_bytes)                                                                               \
+  PDAE_REQUIRE((need) == 0 || ((ws) && (ws_bytes) >= (need)), fn ": workspace of %lld bytes, %lld needed", (long long)(ws_bytes), \
+               (long long)(need))
+
+extern "C" int64_t pdae_conv2d_wgrad_simt_det_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int stride,
+                                                             int pad) {
+  if (!wgrad_simt_shape_ok(B, H, W, Cin, Cout, ksize, stride, pad)) {
+    set_error("conv2d_wgrad_simt_det_workspace_bytes: bad shape");
+    return PDAE_EINVAL;
+  }
+  WgradArgs p;
+  wgrad_simt_args(p, B, H, W, Cin, Cout, ksize, stride, pad);
+  const long long chunks = (p.P + p.chunk - 1) / p.chunk;
+  return chunks > 1 ? chunks * p.MK * Cout * (int64_t)sizeof(float) : 0;
+}
+
+extern "C" int pdae_conv2d_wgrad_simt_det(const float* x, int in_nchw, int a_silu, const float* dy, float* dw_tcico, int B, int H,
+                                          int W, int Cin, int Cout, int ksize, int stride, int pad, float* workspace,
+                                          int64_t workspace_bytes, pdae_stream_t stream) {
+  PDAE_REQUIRE(x && dy && dw_tcico, "conv2d_wgrad_simt_det: null pointer");
+  const int64_t need = pdae_conv2d_wgrad_simt_det_workspace_bytes(B, H, W, Cin, Cout, ksize, stride, pad);
+  if (need < 0) return PDAE_EINVAL;
+  PDAE_DET_WS("conv2d_wgrad_simt_det", need, workspace, workspace_bytes);
+  WgradArgs p;
+  wgrad_simt_args(p, B, H, W, Cin, Cout, ksize, stride, pad);
+  p.x = x; p.dy = dy; p.in_nchw = in_nchw; p.a_silu = a_silu;
+  p.dw = need ? workspace : dw_tcico;
+  const int gz = (int)((p.P + p.chunk - 1) / p.chunk);
+  cudaStream_t s = (cudaStream_t)stream;
+  conv_wgrad_kernel<true><<<dim3(cdiv(p.MK, DBM), cdiv(Cout, DBN), gz), 256, 0, s>>>(p);
+  PDAE_LAUNCH_CHECK("conv_wgrad_kernel<det>");
+  if (need) PDAE_CUDA(launch_slot_sum(workspace, gz, (long long)p.MK * Cout, dw_tcico, s));
+  return PDAE_OK;
+}
+
+extern "C" int64_t pdae_conv2d_dgrad_simt_det_workspace_bytes(int B, int H, int W, int Cin, int Cout, int ksize, int stride,
+                                                             int pad, int accumulate) {
+  if (!wgrad_simt_shape_ok(B, H, W, Cin, Cout, ksize, stride, pad)) {
+    set_error("conv2d_dgrad_simt_det_workspace_bytes: bad shape");
+    return PDAE_EINVAL;
+  }
+  return dgrad_wide_linear(H, W, ksize, stride, pad, Cout, accumulate) ? (int64_t)cdiv(Cout, 64) * B * Cin * sizeof(float) : 0;
+}
+
+// as pdae_conv2d_dgrad_simt; the wide-Linear split-K form stores each 64-row chunk's partial sums in its slot
+extern "C" int pdae_conv2d_dgrad_simt_det(const float* dy, const float* w_tco, float* dx, int B, int H, int W, int Cin, int Cout,
+                                          int ksize, int stride, int pad, int accumulate, float* workspace, int64_t workspace_bytes,
+                                          pdae_stream_t stream) {
+  PDAE_REQUIRE(dy && w_tco && dx, "conv2d_dgrad_simt_det: null pointer");
+  const int64_t need = pdae_conv2d_dgrad_simt_det_workspace_bytes(B, H, W, Cin, Cout, ksize, stride, pad, accumulate);
+  if (need < 0) return PDAE_EINVAL;
+  PDAE_DET_WS("conv2d_dgrad_simt_det", need, workspace, workspace_bytes);
+  if (!need) return pdae_conv2d_dgrad_simt(dy, w_tco, dx, B, H, W, Cin, Cout, ksize, stride, pad, accumulate, stream);
+  cudaStream_t s = (cudaStream_t)stream;
+  linear_dgrad_splitk_kernel<true><<<dim3(cdiv(Cout, 64), cdiv(Cin, 256)), 256, 0, s>>>(dy, w_tco, workspace, B, Cout, Cin);
+  PDAE_LAUNCH_CHECK("linear_dgrad_splitk_kernel<det>");
+  PDAE_CUDA(launch_slot_sum(workspace, cdiv(Cout, 64), (long long)B * Cin, dx, s));
+  return PDAE_OK;
+}
+
+extern "C" int64_t pdae_colsum_det_workspace_bytes(int64_t M, int N) {
+  if (M <= 0 || N <= 0) {
+    set_error("colsum_det_workspace_bytes: M=%lld N=%d must be > 0", (long long)M, N);
+    return PDAE_EINVAL;
+  }
+  const long long chunks = (M + colsum_det_rows(M) - 1) / colsum_det_rows(M);
+  return chunks > 1 ? chunks * N * (int64_t)sizeof(float) : 0;
+}
+
+extern "C" int pdae_colsum_det(const float* dy, int64_t M, int N, float* out, float* workspace, int64_t workspace_bytes,
+                               pdae_stream_t stream) {
+  PDAE_REQUIRE(dy && out, "colsum_det: null pointer");
+  const int64_t need = pdae_colsum_det_workspace_bytes(M, N);
+  if (need < 0) return PDAE_EINVAL;
+  PDAE_DET_WS("colsum_det", need, workspace, workspace_bytes);
+  const long long rows = colsum_det_rows(M);
+  const int chunks = cdiv(M, rows);
+  float* slots = need ? workspace : out;
+  cudaStream_t s = (cudaStream_t)stream;
+  if (N % 4 == 0 && !((uintptr_t)dy & 15)) {
+    colsum_v4_kernel<true><<<chunks, 256, 0, s>>>(dy, M, N, slots, (int)rows);
+    PDAE_LAUNCH_CHECK("colsum_v4_kernel<det>");
+  } else {
+    colsum_kernel<true><<<chunks, N < 256 ? (N < 32 ? 32 : N) : 256, 0, s>>>(dy, M, N, slots, (int)rows);
+    PDAE_LAUNCH_CHECK("colsum_kernel<det>");
+  }
+  if (need) PDAE_CUDA(launch_slot_sum(workspace, chunks, N, out, s));
+  return PDAE_OK;
+}
+
+extern "C" int64_t pdae_gn_bwd_sums_det_workspace_bytes(int B, int H, int W, int C) {
+  if (B <= 0 || H <= 0 || W <= 0 || C <= 0) {
+    set_error("gn_bwd_sums_det_workspace_bytes: B=%d H=%d W=%d C=%d must be > 0", B, H, W, C);
+    return PDAE_EINVAL;
+  }
+  return (int64_t)B * cdiv((long long)H * W, gn_bwd_ppc(B, H * W)) * C * 2 * (int64_t)sizeof(float);
+}
+
+extern "C" int pdae_gn_bwd_sums_det(const float* src1, int C1, const float* src2, int C2, const float* ab, const float* dy,
+                                    int silu, int resample, int B, int H, int W, float* S, float* workspace, int64_t workspace_bytes,
+                                    pdae_stream_t stream) {
+  PDAE_REQUIRE(src1 && ab && dy && S && workspace, "gn_bwd_sums_det: null pointer");
+  if (!src2) C2 = 0;
+  const int C = C1 + C2;
+  PDAE_REQUIRE(C1 % 4 == 0 && C2 % 4 == 0 && C % 32 == 0 && C > 0 && C <= 6144, "gn_bwd_sums_det: bad channels C1=%d C2=%d", C1, C2);
+  PDAE_REQUIRE(resample >= 0 && resample <= 2, "gn_bwd_sums_det: bad resample mode");
+  PDAE_REQUIRE(resample != PDAE_RESAMPLE_DOWN2 || (H % 2 == 0 && W % 2 == 0), "gn_bwd_sums_det: odd dims for DOWN2");
+  const int64_t need = pdae_gn_bwd_sums_det_workspace_bytes(B, H, W, C);
+  if (need < 0) return PDAE_EINVAL;
+  PDAE_DET_WS("gn_bwd_sums_det", need, workspace, workspace_bytes);
+  cudaStream_t s = (cudaStream_t)stream;
+  const int ppc = gn_bwd_ppc(B, H * W), P = cdiv((long long)H * W, ppc);
+  const int L = C / 4, Lb = L < 256 ? L : 256;
+  const size_t sm = (size_t)(256 / Lb) * 2 * C * sizeof(float);
+  dim3 grid(P, B);
+  if (resample == PDAE_RESAMPLE_NONE) gn_bwd_sums_kernel<PDAE_RESAMPLE_NONE, true><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, workspace, ppc);
+  else if (resample == PDAE_RESAMPLE_UP2) gn_bwd_sums_kernel<PDAE_RESAMPLE_UP2, true><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, workspace, ppc);
+  else gn_bwd_sums_kernel<PDAE_RESAMPLE_DOWN2, true><<<grid, 256, sm, s>>>(src1, C1, src2, C2, ab, dy, silu, H, W, workspace, ppc);
+  PDAE_LAUNCH_CHECK("gn_bwd_sums_kernel<det>");
+  PDAE_CUDA(launch_stat_parts_reduce(workspace, B, P, C, S, s));
+  return PDAE_OK;
+}
+
+extern "C" int64_t pdae_gn_bwd_coef_det_workspace_bytes(int B, int C) {
+  if (B <= 0 || C <= 0) {
+    set_error("gn_bwd_coef_det_workspace_bytes: B=%d C=%d must be > 0", B, C);
+    return PDAE_EINVAL;
+  }
+  return (int64_t)2 * B * C * sizeof(float);
+}
+
+extern "C" int pdae_gn_bwd_coef_det(const float* S, const double* sums, const float* gamma, const float* beta, const float* emb,
+                                    int emb_ld, const float* embz, int embz_ld, int B, int C, int HW, float eps, float* kk,
+                                    float* dgamma, float* dbeta, float* demb, int demb_ld, float* dembz, int dembz_ld,
+                                    float* workspace, int64_t workspace_bytes, pdae_stream_t stream) {
+  PDAE_REQUIRE(S && sums && gamma && beta && kk, "gn_bwd_coef_det: null pointer");
+  PDAE_REQUIRE(C % 32 == 0 && C <= 2048, "gn_bwd_coef_det: C=%d (a multiple of 32, <= 2048)", C);
+  const int64_t need = (dgamma || dbeta) ? pdae_gn_bwd_coef_det_workspace_bytes(B, C) : 0;
+  if (need < 0) return PDAE_EINVAL;
+  PDAE_DET_WS("gn_bwd_coef_det", need, workspace, workspace_bytes);
+  cudaStream_t s = (cudaStream_t)stream;
+  gn_bwd_coef_kernel<true><<<B, C < 1024 ? (C < 32 ? 32 : C) : 1024, (size_t)2 * C * sizeof(double), s>>>(
+      S, sums, gamma, beta, emb, emb_ld, embz, embz_ld, C, HW, eps, kk, dgamma ? workspace : nullptr,
+      dbeta ? workspace + (long long)B * C : nullptr, demb, demb_ld, dembz, dembz_ld);
+  PDAE_LAUNCH_CHECK("gn_bwd_coef_kernel<det>");
+  if (need) {
+    gn_param_reduce_kernel<<<cdiv(C, 256), 256, 0, s>>>(workspace, B, C, dgamma, dbeta);
+    PDAE_LAUNCH_CHECK("gn_param_reduce_kernel");
+  }
+  return PDAE_OK;
+}
+
+extern "C" int pdae_embedding_bwd_det(const float* d_emb, const int64_t* idx, float* dw, int B, int E, int rows,
+                                      pdae_stream_t stream) {
+  PDAE_REQUIRE(d_emb && idx && dw && B > 0 && E > 0 && rows > 0, "embedding_bwd_det: bad args");
+  embedding_bwd_det_kernel<<<cdiv((long long)rows * E, 256), 256, 0, (cudaStream_t)stream>>>(d_emb, idx, dw, B, E, rows);
+  PDAE_LAUNCH_CHECK("embedding_bwd_det_kernel");
   return PDAE_OK;
 }

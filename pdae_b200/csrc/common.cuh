@@ -13,6 +13,8 @@ void set_error(const char* fmt, ...);
 // Deterministic statistics (norm_elementwise.cu): per-channel (sum, sum^2) partials [B][P][C][2], written with plain stores by
 // P producers per image, summed over P in ascending order into [B][C][2].
 cudaError_t launch_stat_parts_reduce(const float* part, int B, int P, int C, float* chs, cudaStream_t s);
+// out[i] = sum over s = 0..S-1, in that order, of part[s * n + i] (backward_simt.cu): the reduction of deterministic slots
+cudaError_t launch_slot_sum(const float* part, int S, long long n, float* out, cudaStream_t s);
 
 #define PDAE_REQUIRE(cond, ...)             \
   do {                                      \

@@ -42,7 +42,9 @@
 // image stores its per-channel sums in the tile's own slot [B][tiles per image][Cout][2] (plain stores; the run then sums the
 // slots in order); a tile holding several whole images sums each (image, column) with one thread, in row order, straight into
 // [B][Cout][2].  Split-K: item (tile, split) stores its partial tile in slot [split][B][Cout] and the run adds the splits in
-// order, then the bias; the split count follows K and N alone.
+// order, then the bias; the split count follows K and N alone.  The training GEMMs (GM_A_MN / GM_B_MN, the softmax-gradient
+// epilogue) and the stride-2 data gradient record no statistics, yet their default instantiations still compile the atomic
+// statistics flush; their DET instantiations are the same kernels with that code compiled out.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -1303,7 +1305,10 @@ static int tc2_det_splitk(const pdae_conv_tc2_plan* pl, int* kchunk) {
   return (pl->args.kblocks + kc - 1) / kc;
 }
 
-static bool tc2_det_mode_ok(const pdae_conv_tc2_plan* pl) { return pl->gm == GM_SPLITK || (pl->gm == 0 && pl->s2 != 2); }
+static bool tc2_det_mode_ok(const pdae_conv_tc2_plan* pl) {
+  if (pl->gm == GM_SPLITK || (pl->gm == 0 && pl->s2 != 2)) return true;
+  return pl->args.ch_stats == nullptr;   // training GEMMs and the stride-2 data gradient: no statistics, nothing to slot
+}
 
 extern "C" int64_t pdae_conv_tc2_det_workspace_bytes(const pdae_conv_tc2_plan* pl) {
   if (!pl) {
@@ -1366,7 +1371,14 @@ extern "C" int pdae_conv_tc2_run(const pdae_conv_tc2_plan* pl, pdae_stream_t str
         splitk_reduce_kernel<<<cdiv(n, 256), 256, 0, s>>>(a.out_nchw, a.splitk, n, a.Cout, a.bias, pl->det_out);
         e = cudaPeekAtLastError();
       }
-    } else {
+    } else if (pl->gm == (GM_SMGRAD | GM_SPLITN)) e = T2_GO_DET(128, true, 0, GM_SMGRAD | GM_SPLITN);
+    else if (pl->gm == GM_SMGRAD) e = pl->BN == 128 ? T2_GO_DET(128, true, 0, GM_SMGRAD) : T2_GO_DET(64, true, 0, GM_SMGRAD);
+    else if (pl->gm == GM_A_MN) e = pl->BN == 128 ? T2_GO_DET(128, false, 0, GM_A_MN) : T2_GO_DET(64, false, 0, GM_A_MN);
+    else if (pl->gm == GM_B_MN) e = pl->BN == 128 ? T2_GO_DET(128, false, 0, GM_B_MN) : T2_GO_DET(64, false, 0, GM_B_MN);
+    else if (pl->gm == (GM_A_MN | GM_B_MN))
+      e = pl->BN == 128 ? T2_GO_DET(128, false, 0, GM_A_MN | GM_B_MN) : T2_GO_DET(64, false, 0, GM_A_MN | GM_B_MN);
+    else if (pl->s2 == 2) e = pl->BN == 128 ? T2_GO_DET(128, false, 2, 0) : T2_GO_DET(64, false, 2, 0);
+    else {
       if (pl->s2 == 1) e = pl->BN == 128 ? (ob ? T2_GO_DET(128, true, 1, 0) : T2_GO_DET(128, false, 1, 0))
                                          : (ob ? T2_GO_DET(64, true, 1, 0) : T2_GO_DET(64, false, 1, 0));
       else switch (pl->BN) {

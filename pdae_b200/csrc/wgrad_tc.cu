@@ -30,6 +30,12 @@
 // the OUTPUT grid (dY is read there, unshifted); the activation is read through its parity view [B][H/2][2][W/2][2C]
 // (conv_tc2.cu): tap (ky, kx) is the parity class (ky != 1, kx != 1) at the output tile shifted by -1 where the tap index is
 // 0, the -1 coordinate being zero-filled by TMA (the padding).
+//
+// DET (pdae_wgrad_tc_set_deterministic): no float atomics.  Work unit = (group, pixel split), one per CTA: split s of a group
+// covers k-tiles [s kpt, s kpt + kpt) and stores its partial tile with plain stores into slot s of a caller-owned workspace
+// [splits][taps][Cin][Cout]; the run then adds the slots in split order into dW.  The split count follows the shape alone
+// (the least estimated time of the units on a 132-SM H100 SXM, wg_det_splits), so the sums do not depend on the GPU; with one
+// split a unit stores straight into dW.
 #include <cuda.h>
 
 #include "common.cuh"
@@ -55,6 +61,8 @@ struct WgradArgs {
   int B, H, W;
   int stages;
   long long items;          // taps * mchunks * nchunks * ktiles
+  int det_splits, det_kpt;  // DET: pixel splits per group and k-tiles per split
+  long long det_slot;       // DET: elements of one slot (= of dW)
 };
 
 namespace wg {
@@ -109,7 +117,7 @@ __device__ __forceinline__ bool elect_one() {
 }
 }  // namespace wg
 
-template <int BN, bool SPLIT, bool S2 = false>
+template <int BN, bool SPLIT, bool S2 = false, bool DET = false>
 __global__ void __launch_bounds__(WG_THREADS, 1)
 wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, WgradArgs p) {
   using namespace wg;
@@ -126,8 +134,11 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
   const int S = p.stages;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const long long per_cta = (p.items + gridDim.x - 1) / gridDim.x;
-  const long long it_begin = (long long)blockIdx.x * per_cta;
-  const long long it_end = it_begin + per_cta < p.items ? it_begin + per_cta : p.items;
+  // DET: blockIdx.x = group * det_splits + split
+  const long long det_g = DET ? blockIdx.x / p.det_splits : 0, det_s = DET ? blockIdx.x - det_g * p.det_splits : 0;
+  const long long it_begin = DET ? det_g * p.ktiles + det_s * p.det_kpt : (long long)blockIdx.x * per_cta;
+  const long long it_end = DET ? det_g * p.ktiles + min((long long)p.ktiles, (det_s + 1) * p.det_kpt)
+                               : (it_begin + per_cta < p.items ? it_begin + per_cta : p.items);
 
   if (threadIdx.x == 0) {
     for (int s = 0; s < S; ++s) {
@@ -217,12 +228,14 @@ wgrad_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
       const int tap = gg / p.mchunks;
       const int tap_w = p.pair ? 2 * tap + wgi : tap;             // pair mode: rows 64-127 belong to the second tap
       if (tap_w >= p.taps) return;
-      float* base = p.dw + (long long)tap_w * p.stap + (long long)(nc * BN) * p.sn;
+      float* base = p.dw + det_s * p.det_slot + (long long)tap_w * p.stap + (long long)(nc * BN) * p.sn;
 #pragma unroll
       for (int i = 0; i < BN / 2; ++i) {
         const int m = wgmma::frag_row(t, i);
         const int ch_m = p.pair ? mc * 64 + m : mc * 128 + 64 * wgi + m;
-        atomicAdd(base + (long long)ch_m * p.sm + (long long)wgmma::frag_col(t, i) * p.sn, acc[i]);
+        float* o = base + (long long)ch_m * p.sm + (long long)wgmma::frag_col(t, i) * p.sn;
+        if constexpr (DET) *o = acc[i];
+        else atomicAdd(o, acc[i]);
       }
     };
     int s = 0;
@@ -291,15 +304,15 @@ static int pow2_tile_w(int W, int cap) {
   return t;
 }
 
-template <int BN, bool SPLIT, bool S2 = false>
+template <int BN, bool SPLIT, bool S2 = false, bool DET = false>
 static cudaError_t launch_wg(const CUtensorMap& a, const CUtensorMap& b, const WgradArgs& args, int grid, size_t smem, cudaStream_t s) {
   static bool attr_set = false;
   if (!attr_set) {
-    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<BN, SPLIT, S2>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
+    cudaError_t e = cudaFuncSetAttribute(wgrad_tc_kernel<BN, SPLIT, S2, DET>, cudaFuncAttributeMaxDynamicSharedMemorySize, 221 * 1024);
     if (e != cudaSuccess) return e;
     attr_set = true;
   }
-  wgrad_tc_kernel<BN, SPLIT, S2><<<grid, WG_THREADS, smem, s>>>(a, b, args);
+  wgrad_tc_kernel<BN, SPLIT, S2, DET><<<grid, WG_THREADS, smem, s>>>(a, b, args);
   return cudaPeekAtLastError();
 }
 
@@ -313,6 +326,8 @@ struct pdae_wgrad_tc_plan {
   int BN, split, grid;
   int s2;           // stride-2 3x3 conv (wgrad_tc_kernel's S2)
   size_t smem;
+  int det;          // pdae_wgrad_tc_set_deterministic: the DET kernel
+  float* det_out;   // DET with several splits: dW, which the run sums the slots into (args.dw is then the workspace)
 };
 
 static int g_num_sms_w = 0;
@@ -427,11 +442,68 @@ extern "C" int pdae_wgrad_tc_create_bf16_s2(pdae_wgrad_tc_plan** plan_out, const
   return wgrad_create(plan_out, act_bf16, dy_bf16, dw, B, H, W, Cin, Cout, 3, false, true);
 }
 
+// ---- deterministic plans (kernel header, DET) ----------------------------------------------------------------------------
+constexpr int WG_DET_SMS = 132;   // SMs of an H100 SXM: a constant, so that the split count follows the shape alone
+
+// The split count with the least estimated time on WG_DET_SMS SMs running one unit each: waves x k-tiles per unit, plus the
+// slot traffic (each split writes and the reduction reads one dW image: about n / 750000 k-tile times of a split-operand
+// unit at HBM speed, three times that for the single-pass bf16 unit, whose k-tile is a third of the work).
+static int wg_det_splits(const WgradArgs& a, int split, int* kpt) {
+  const long long groups = a.items / a.ktiles, n = (long long)a.taps * a.stap;
+  double best = 0.0;
+  int bk = a.ktiles;
+  for (int s = 1; s <= a.ktiles; ++s) {
+    const int k = (a.ktiles + s - 1) / s;
+    if (s > 1 && (a.ktiles + k - 1) / k != s) continue;                 // every split non-empty
+    const double waves = (double)((groups * s + WG_DET_SMS - 1) / WG_DET_SMS);
+    const double cost = waves * k + (s > 1 ? (double)s * n / 750000.0 * (split ? 1 : 3) : 0.0);
+    if (s == 1 || cost < best) { best = cost; bk = k; }
+  }
+  if (kpt) *kpt = bk;
+  return (a.ktiles + bk - 1) / bk;
+}
+
+extern "C" int64_t pdae_wgrad_tc_det_workspace_bytes(const pdae_wgrad_tc_plan* pl) {
+  if (!pl) {
+    set_error("wgrad_tc_det_workspace_bytes: null plan");
+    return PDAE_EINVAL;
+  }
+  const int splits = wg_det_splits(pl->args, pl->split, nullptr);
+  return splits > 1 ? (int64_t)splits * pl->args.taps * pl->args.stap * (int64_t)sizeof(float) : 0;
+}
+
+extern "C" int pdae_wgrad_tc_set_deterministic(pdae_wgrad_tc_plan* pl, float* workspace, int64_t workspace_bytes) {
+  PDAE_REQUIRE(pl, "wgrad_tc_set_deterministic: null plan");
+  PDAE_REQUIRE(!pl->det, "wgrad_tc_set_deterministic: the plan is deterministic already");
+  const int64_t need = pdae_wgrad_tc_det_workspace_bytes(pl);
+  PDAE_REQUIRE(workspace_bytes >= need && (need == 0 || workspace),
+               "wgrad_tc_set_deterministic: workspace of %lld bytes, %lld needed (pdae_wgrad_tc_det_workspace_bytes)",
+               (long long)workspace_bytes, (long long)need);
+  PDAE_REQUIRE(!((uintptr_t)workspace & 3), "wgrad_tc_set_deterministic: workspace must be 4-byte aligned");
+  WgradArgs& a = pl->args;
+  a.det_splits = wg_det_splits(a, pl->split, &a.det_kpt);
+  a.det_slot = (long long)a.taps * a.stap;
+  pl->grid = (int)(a.items / a.ktiles) * a.det_splits;
+  if (need > 0) {
+    pl->det_out = a.dw;
+    a.dw = workspace;
+  }
+  pl->det = 1;
+  return PDAE_OK;
+}
+
 extern "C" int pdae_wgrad_tc_run(const pdae_wgrad_tc_plan* pl, pdae_stream_t stream) {
   PDAE_REQUIRE(pl, "wgrad_tc_run: null plan");
   cudaStream_t s = (cudaStream_t)stream;
   cudaError_t e;
-  if (pl->s2)
+  if (pl->det) {
+#define WG_DET(BN, SPLIT, S2) launch_wg<BN, SPLIT, S2, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s)
+    if (pl->s2) e = pl->BN == 128 ? WG_DET(128, false, true) : WG_DET(64, false, true);
+    else if (pl->split) e = pl->BN == 128 ? WG_DET(128, true, false) : WG_DET(64, true, false);
+    else e = pl->BN == 128 ? WG_DET(128, false, false) : WG_DET(64, false, false);
+#undef WG_DET
+    if (e == cudaSuccess && pl->det_out) e = launch_slot_sum(pl->args.dw, pl->args.det_splits, pl->args.det_slot, pl->det_out, s);
+  } else if (pl->s2)
     e = pl->BN == 128 ? launch_wg<128, false, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s)
                       : launch_wg<64, false, true>(pl->tmA, pl->tmB, pl->args, pl->grid, pl->smem, s);
   else if (pl->split)

@@ -18,7 +18,9 @@ Precision modes
 Deterministic plans (``Plan(..., deterministic=True)``; the modules record them while
 ``torch.are_deterministic_algorithms_enabled()``): every cross-CTA reduction -- GroupNorm statistics, split-K Linears -- runs
 on kernels without float atomics whose partial results have fixed slots summed in a fixed order, so a replay gives the same
-bits for the same inputs.  The default plans keep the atomic kernels.
+bits for the same inputs.  The default plans keep the atomic kernels.  A deterministic backward plan (train.py) does the same for
+the weight / bias / GroupNorm / embedding gradients and the split-K data gradients; every gradient buffer is then written by
+plain stores (Plan.new_grad), so it needs no zeroed accumulator.
 """
 from __future__ import annotations
 
@@ -109,9 +111,22 @@ class Packed:
         version counter, so every sampling loop / graph capture forces one refresh (Plan.run_prologue)."""
         st = self._stamp()
         if force or st != self.stamp:
-            with torch.inference_mode(False), torch.no_grad():
+            with torch.inference_mode(False), torch.no_grad(), _fully_written():
                 self.tensor.copy_(self.fn())
             self.stamp = st
+
+
+class _fully_written:
+    """Within: PyTorch does not fill new tensors first (torch.utils.deterministic.fill_uninitialized_memory, which the
+    deterministic mode turns on).  A pack's temporaries are written in full by the ops that make them, and a training step
+    re-packs every updated weight: the fill would add a kernel per temporary, several hundred per step."""
+
+    def __enter__(self):
+        self.was = torch.utils.deterministic.fill_uninitialized_memory
+        torch.utils.deterministic.fill_uninitialized_memory = False
+
+    def __exit__(self, *exc):
+        torch.utils.deterministic.fill_uninitialized_memory = self.was
 
 
 def split3_weights(w: torch.Tensor) -> torch.Tensor:
@@ -182,6 +197,7 @@ class Plan:
         self._stats_elems = 0
         self.graph = None
         self.flops: List[float] = []  # algorithmic FLOPs (2*MACs) per recorded op, 0 for non-contraction ops
+        self._launches: Dict[int, int] = {}   # op index -> kernel launches, where the op's shape decides it (Plan.call)
 
     # ---- buffers ----------------------------------------------------------------------------
     def new(self, shape, dtype=torch.float32, name="") -> Buf:
@@ -197,6 +213,20 @@ class Plan:
         off = self._stats_elems
         self._stats_elems += int(nelems)
         return BufView(self._stats_arena, off)
+
+    def new_grad(self, nelems: int) -> "BufView":
+        """fp32 gradient buffer of `nelems` elements: in the zeroed arena (new_zeroed) for the atomic kernels of a default plan;
+        private storage, written by plain stores and read after the run, in a deterministic plan."""
+        if not self.det:
+            return self.new_zeroed(nelems)
+        b = self.new((int(nelems),), torch.float32, "grad")
+        b.keep = True
+        return BufView(b, 0)
+
+    def det_workspace(self, nbytes: int, what: str) -> Buf:
+        """Arena scratch for the slots of a deterministic op (`nbytes` from its *_workspace_bytes query)."""
+        _native.check(min(int(nbytes), 0), what)
+        return self.new((max(int(nbytes), 16) // 4,), torch.float32, "det_slots")
 
     def fixed(self, t: torch.Tensor) -> Buf:
         assert t.is_contiguous(), "plan tensors must be contiguous"
@@ -238,8 +268,11 @@ class Plan:
                 plan._in_prologue = False
         return _Ctx()
 
-    def call(self, fn: str, *args, flops: float = 0.0) -> None:
+    def call(self, fn: str, *args, flops: float = 0.0, launches: Optional[int] = None) -> None:
+        """Record one native call.  launches: the kernels it runs when that depends on its shape (otherwise _LAUNCHES / 1)."""
         idx = len(self.ops)
+        if launches is not None:
+            self._launches[idx] = int(launches)
         self.flops.append(float(flops))
         self.op_pro.append(self._in_prologue)
         flat = []
@@ -264,6 +297,7 @@ class Plan:
             self.ops.insert(0, ("zero", [self._stats_arena, ctypes.c_int64(self._stats_elems * 4), _STREAM]))
             self.flops.insert(0, 0.0)
             self.op_pro.insert(0, False)
+            self._launches = {i + 1: n for i, n in self._launches.items()}
             for b in self.bufs:  # op indices shift by one
                 if b is not self._stats_arena and b.first is not None:
                     b.first += 1
@@ -311,10 +345,8 @@ class Plan:
         compiled = []
         for fn, args in self.ops:
             if self.det and fn in DET_OPS:   # the handle each of these ops compiles to is switched to its DET kernels below
-                tc3 = fn == "conv_tc3"
-                self._det_handles.append((len(compiled),
-                                          self.L.pdae_conv_tc3_set_deterministic if tc3 else self.L.pdae_conv_tc2_set_deterministic,
-                                          self.L.pdae_conv_tc3_det_workspace_bytes if tc3 else self.L.pdae_conv_tc2_det_workspace_bytes))
+                setter, query = det_entry_points(fn)
+                self._det_handles.append((len(compiled), getattr(self.L, setter), getattr(self.L, query)))
             if fn == "conv_tc2":
                 compiled.append(self._compile_tc2(args))
                 continue
@@ -378,8 +410,8 @@ class Plan:
         for b in self.bufs:  # a recycled buffer must not carry data from the prologue into the per-step ops
             if b.first is not None and not b.keep and not b.fixed and self.op_pro[b.first] and not self.op_pro[b.last]:
                 raise AssertionError(f"plan buffer {b.name!r} crosses the prologue boundary but is not `keep`")
-        self.n_launch = sum(_LAUNCHES.get(fn, 1) + extra.get(i, 0) for i, ((fn, _), p) in enumerate(zip(self.ops, self.op_pro))
-                            if not p)
+        self.n_launch = sum(self._launches.get(i, _LAUNCHES.get(fn, 1)) + extra.get(i, 0)
+                            for i, ((fn, _), p) in enumerate(zip(self.ops, self.op_pro)) if not p)
         return self
 
     @staticmethod
@@ -1057,13 +1089,24 @@ class Plan:
         return act, raw
 
 
-# Tensor-core ops a deterministic plan switches to their DET kernels at finalize (pdae_conv_tc2/tc3_set_deterministic).
-DET_OPS = frozenset({"conv_tc2", "conv_tc2_skip", "conv_tc2_s2", "conv_tc2_splitk", "gemm_tc2", "gemm_tc2_softmax", "conv_tc3"})
+# Tensor-core ops a deterministic plan switches to their DET kernels at finalize (pdae_conv_tc2 / tc3 / wgrad_tc
+# _set_deterministic).  The training GEMMs and the stride-2 data gradient record no statistics; their DET kernels are the same
+# kernels without the compiled-in atomic statistics code (conv_tc2.cu).
+DET_OPS = frozenset({"conv_tc2", "conv_tc2_skip", "conv_tc2_s2", "conv_tc2_splitk", "gemm_tc2", "gemm_tc2_softmax", "conv_tc3",
+                     "gemm_tc2_major", "gemm_tc2_softmax_grad", "conv_tc2_s2_dgrad", "wgrad_tc", "wgrad_tc_bf16",
+                     "wgrad_tc_bf16_s2"})
+
+
+def det_entry_points(fn: str) -> Tuple[str, str]:
+    """(set_deterministic, det_workspace_bytes) entry points of the handle an op of DET_OPS compiles to."""
+    kind = "conv_tc3" if fn == "conv_tc3" else ("wgrad_tc" if fn.startswith("wgrad_tc") else "conv_tc2")
+    return f"pdae_{kind}_set_deterministic", f"pdae_{kind}_det_workspace_bytes"
+
+
 # Ops whose kernels reduce with float atomics (or accumulate into a zeroed buffer): never in a deterministic plan, whose
-# recording uses the *_det ops instead (training-only ops are listed too: a deterministic plan is forward-only).
-NONDET_OPS = frozenset({"zero", "ch_stats", "gn_stats", "stem_conv_bf16", "stem_conv_s2_bf16", "conv_tc2_s2_dgrad",
-                        "gemm_tc2_major", "gemm_tc2_softmax_grad", "wgrad_tc", "wgrad_tc_bf16", "wgrad_tc_bf16_s2",
-                        "conv2d_wgrad_simt", "conv2d_dgrad_simt", "gn_bwd_sums", "gn_bwd_coef", "colsum", "embedding_bwd",
-                        "mlp_mod_ln_act_bwd", "mlp_mod_ln_act_bwd_bf16"})
+# recording uses the *_det ops instead.
+NONDET_OPS = frozenset({"zero", "ch_stats", "gn_stats", "stem_conv_bf16", "stem_conv_s2_bf16", "conv2d_wgrad_simt",
+                        "conv2d_dgrad_simt", "gn_bwd_sums", "gn_bwd_coef", "colsum", "embedding_bwd", "mlp_mod_ln_act_bwd",
+                        "mlp_mod_ln_act_bwd_bf16"})
 
 _LAUNCHES = {"gn_stats": 1, "attention_simt": 3, "zero": 0, "ch_stats_det": 2, "gn_stats_det": 2, "stem_conv_bf16_det": 2}

@@ -117,11 +117,12 @@ def draw_dropout_masks(plan: Plan) -> None:
         mask.tensor.bernoulli_(1.0 - p)
 
 
-def bwd_plan(dev, amp: bool = False) -> Plan:
+def bwd_plan(dev, amp: bool = False, det: bool = False) -> Plan:
     """Backward plans are tensor-core plans: the data gradient of every eligible stride-1 conv runs on `conv_tc2` and its
     weight gradient on `wgrad_tc`, both in the fp32-grade split-operand "bf16x3" mode, or with `amp` in the single-pass
-    "bf16" mode (Backward.conv); everything else in them is fp32 CUDA-core arithmetic."""
-    return Plan(dev, "bf16" if amp else "bf16x3")
+    "bf16" mode (Backward.conv); everything else in them is fp32 CUDA-core arithmetic.  `det`: the deterministic plan
+    (torch.use_deterministic_algorithms): DET tensor-core kernels and the *_det CUDA-core reductions, no float atomics."""
+    return Plan(dev, "bf16" if amp else "bf16x3", deterministic=det)
 
 
 def autocast_active() -> bool:
@@ -150,6 +151,36 @@ class Backward:
             self._fixed[k] = self.P.fixed(b.tensor)
         return self._fixed[k]
 
+    # ---- CUDA-core reductions: the atomic kernels, or in a deterministic plan their *_det forms (slots summed in order) --
+    def wgrad_simt(self, x, in_nchw: int, a_silu: int, dy, dw, B, H, W, Cin, Cout, k, stride, pad) -> None:
+        P = self.P
+        if not P.det:
+            P.call("conv2d_wgrad_simt", x, in_nchw, a_silu, dy, dw, B, H, W, Cin, Cout, k, stride, pad, _STREAM)
+            return
+        n = P.L.pdae_conv2d_wgrad_simt_det_workspace_bytes(B, H, W, Cin, Cout, k, stride, pad)
+        ws = P.det_workspace(n, "pdae_conv2d_wgrad_simt_det_workspace_bytes")
+        P.call("conv2d_wgrad_simt_det", x, in_nchw, a_silu, dy, dw, B, H, W, Cin, Cout, k, stride, pad, ws,
+               ctypes.c_int64(ws.nbytes), _STREAM, launches=2 if n else 1)
+
+    def dgrad_simt(self, dy, wt, dx, B, H, W, Cin, Cout, k, stride, pad) -> None:
+        P = self.P
+        if not P.det:
+            P.call("conv2d_dgrad_simt", dy, wt, dx, B, H, W, Cin, Cout, k, stride, pad, 0, _STREAM)
+            return
+        n = P.L.pdae_conv2d_dgrad_simt_det_workspace_bytes(B, H, W, Cin, Cout, k, stride, pad, 0)
+        ws = P.det_workspace(n, "pdae_conv2d_dgrad_simt_det_workspace_bytes")
+        P.call("conv2d_dgrad_simt_det", dy, wt, dx, B, H, W, Cin, Cout, k, stride, pad, 0, ws, ctypes.c_int64(ws.nbytes), _STREAM,
+               launches=2 if n else 1)
+
+    def colsum(self, dy, M: int, N: int, out) -> None:
+        P = self.P
+        if not P.det:
+            P.call("colsum", dy, ctypes.c_int64(M), N, out, _STREAM)
+            return
+        n = P.L.pdae_colsum_det_workspace_bytes(M, N)
+        ws = P.det_workspace(n, "pdae_colsum_det_workspace_bytes")
+        P.call("colsum_det", dy, ctypes.c_int64(M), N, out, ws, ctypes.c_int64(ws.nbytes), _STREAM, launches=2 if n else 1)
+
     # ---- conv / linear ------------------------------------------------------------------------------------------
     def conv(self, x, dy: Buf, weight: torch.Tensor, bias: Optional[torch.Tensor], *, B, H, W, Cin, Cout, k, stride=1, pad=None,
              need_dx=True, in_nchw=False, a_silu=False, trainable=True, w_unpack=None) -> Optional[Buf]:
@@ -167,7 +198,7 @@ class Backward:
         ce = 3 if P.x3 else 1
         dy3 = None
         if trainable:
-            dw = P.new_zeroed(kk * Cin * Cout)
+            dw = P.new_grad(kk * Cin * Cout)
             if s2:
                 act = getattr(x, "tc_copy", None)     # left by the bf16 training forward (Plan.conv)
                 if act is not None and tuple(act.shape) == (B, H, W, Cin):
@@ -191,13 +222,12 @@ class Backward:
                 P.call("wgrad_tc" if P.x3 else "wgrad_tc_bf16", a3, dy3, dw, B, H, W, Cin, Cout, k,
                        flops=2.0 * B * H * W * Cin * Cout * kk)
             else:
-                P.call("conv2d_wgrad_simt", self.fx(x), int(in_nchw), int(a_silu), dy, dw, B, H, W, Cin, Cout, k, stride, pad,
-                       _STREAM)
+                self.wgrad_simt(self.fx(x), int(in_nchw), int(a_silu), dy, dw, B, H, W, Cin, Cout, k, stride, pad)
             unpack = w_unpack or (lambda t, kk=kk, Cin=Cin, Cout=Cout: t.view(kk, Cin, Cout).permute(2, 1, 0))
             self.sink.add(weight, dw, kk * Cin * Cout, unpack)
             if bias is not None:
-                db = P.new_zeroed(Cout)
-                P.call("colsum", dy, ctypes.c_int64(B * Ho * Wo), Cout, db, _STREAM)
+                db = P.new_grad(Cout)
+                self.colsum(dy, B * Ho * Wo, Cout, db)
                 self.sink.add(bias, db, Cout, lambda t: t)
         if not need_dx:
             return None
@@ -224,7 +254,7 @@ class Backward:
             return dx
         wt = P.pack((id(weight), "tco"), [weight], lambda: weight.detach().reshape(Cout, Cin, kk).permute(2, 0, 1).float())
         dx = P.new((B, H, W, Cin), torch.float32, "dx")
-        P.call("conv2d_dgrad_simt", dy, wt, dx, B, H, W, Cin, Cout, k, stride, pad, 0, _STREAM)
+        self.dgrad_simt(dy, wt, dx, B, H, W, Cin, Cout, k, stride, pad)
         return dx
 
     # ---- GroupNorm (+AdaGN) + SiLU (+resample) --------------------------------------------------------------------
@@ -236,19 +266,30 @@ class Backward:
         B, H, W, C1, C2 = src.B, src.H, src.W, src.C1, src.C2
         C = C1 + C2
         S = P.new((B, C, 2), torch.float32, "gn_bwd_S")
-        P.call("gn_bwd_sums", self.fx(src.b1), C1, self.fx(src.b2), C2, self.fx(ab), dy, int(silu), resample, B, H, W, S, _STREAM)
+        if P.det:
+            ws = P.det_workspace(P.L.pdae_gn_bwd_sums_det_workspace_bytes(B, H, W, C), "pdae_gn_bwd_sums_det_workspace_bytes")
+            P.call("gn_bwd_sums_det", self.fx(src.b1), C1, self.fx(src.b2), C2, self.fx(ab), dy, int(silu), resample, B, H, W, S,
+                   ws, ctypes.c_int64(ws.nbytes), _STREAM, launches=2)
+        else:
+            P.call("gn_bwd_sums", self.fx(src.b1), C1, self.fx(src.b2), C2, self.fx(ab), dy, int(silu), resample, B, H, W, S,
+                   _STREAM)
         kk = P.new((B, 3, C), torch.float32, "gn_bwd_k")
         dg = db = None
         if trainable:
-            dg, db = P.new_zeroed(C), P.new_zeroed(C)
+            dg, db = P.new_grad(C), P.new_grad(C)
             self.sink.add(gn_mod.weight, dg, C, lambda t: t)
             self.sink.add(gn_mod.bias, db, C, lambda t: t)
         e, eld = (self.fx(emb[0]).at(emb[1]), emb[2]) if emb is not None else (None, 0)
         z, zld = (self.fx(embz[0]).at(embz[1]), embz[2]) if embz is not None else (None, 0)
         de, deld = (demb[0].at(demb[1]), demb[2]) if demb is not None else (None, 0)
         dz, dzld = (dembz[0].at(dembz[1]), dembz[2]) if dembz is not None else (None, 0)
-        P.call("gn_bwd_coef", S, self.fx(sums), P.param(gn_mod.weight), P.param(gn_mod.bias), e, eld, z, zld, B, C, H * W, F32(1e-5),
-               kk, dg, db, de, deld, dz, dzld, _STREAM)
+        coef = (S, self.fx(sums), P.param(gn_mod.weight), P.param(gn_mod.bias), e, eld, z, zld, B, C, H * W, F32(1e-5), kk, dg, db,
+                de, deld, dz, dzld)
+        if P.det:
+            ws = P.det_workspace(P.L.pdae_gn_bwd_coef_det_workspace_bytes(B, C), "pdae_gn_bwd_coef_det_workspace_bytes")
+            P.call("gn_bwd_coef_det", *coef, ws, ctypes.c_int64(ws.nbytes), _STREAM, launches=2 if trainable else 1)
+        else:
+            P.call("gn_bwd_coef", *coef, _STREAM)
         dx = P.new((B, H, W, C1), torch.float32, "gn_dx")
         dx2 = P.new((B, H, W, C2), torch.float32, "gn_dx_skip") if (want_dx2 and C2) else None
         P.call("gn_bwd_apply", self.fx(src.b1), C1, self.fx(src.b2), C2, self.fx(ab), kk, dy, int(silu), resample, B, H, W, add,
@@ -345,10 +386,10 @@ class Backward:
                     need_dx: bool) -> Optional[Buf]:
         """Backward of  bank = Linear_cat(SiLU(emb_in)) : per-block weight/bias grads, and (optionally) d emb_in."""
         P = self.P
-        dw = P.new_zeroed(E * total)
-        P.call("conv2d_wgrad_simt", self.fx(emb_in), 0, 1, d_bank, dw, B, 1, 1, E, total, 1, 1, 0, _STREAM)
-        db = P.new_zeroed(total)
-        P.call("colsum", d_bank, ctypes.c_int64(B), total, db, _STREAM)
+        dw = P.new_grad(E * total)
+        self.wgrad_simt(self.fx(emb_in), 0, 1, d_bank, dw, B, 1, 1, E, total, 1, 1, 0)
+        db = P.new_grad(total)
+        self.colsum(d_bank, B, total, db)
         for lin, off in zip(lins, offsets):
             n = lin.weight.shape[0]
             self.sink.add(lin.weight, dw, E * total, lambda t, off=off, n=n: t.view(E, total)[:, off:off + n].t())
@@ -358,7 +399,7 @@ class Backward:
         ws = [l.weight for l in lins]
         wt = P.pack(("bank_tco", id(ws[0])), ws, lambda: torch.cat([w.detach() for w in ws], dim=0).float())  # [total][E]
         g = P.new((B, E), torch.float32, "d_silu_emb")
-        P.call("conv2d_dgrad_simt", d_bank, wt, g, B, 1, 1, E, total, 1, 1, 0, 0, _STREAM)
+        self.dgrad_simt(d_bank, wt, g, B, 1, 1, E, total, 1, 1, 0)
         dx = P.new((B, E), torch.float32, "d_emb")
         P.call("dsilu_mul", g, self.fx(emb_in), dx, ctypes.c_int64(B * E), _STREAM)
         return dx
@@ -376,11 +417,12 @@ class _Generation:
     _gen = 0
     _consumed = -1
     _det_warned = False
+    _det_supported = True   # the trainer records deterministic plans under torch.use_deterministic_algorithms
 
     def _stamp(self) -> int:
-        if torch.are_deterministic_algorithms_enabled() and not self._det_warned:
-            # the training plans keep their atomic reductions (weight gradients, GroupNorm backward): say so once, do not raise,
-            # so that a training run with the switch on keeps working
+        if not self._det_supported and torch.are_deterministic_algorithms_enabled() and not self._det_warned:
+            # this trainer keeps its atomic reductions under the switch: say so once, do not raise, so that a training run with
+            # the switch on keeps working
             self._det_warned = True
             warnings.warn(f"pdae_b200 {type(self).__name__}: the training forward/backward has no deterministic implementation "
                           "yet; torch.use_deterministic_algorithms covers the pdae_b200 forward-only and sampling paths only",
@@ -403,9 +445,10 @@ class ShiftUNetTrainer(_Generation):
     """Forward (fp32, all intermediates kept) + backward plans of a ShiftUNet for one input shape; `amp`: the bf16 plans of
     a forward under autocast (module docstring)."""
 
-    def __init__(self, net, B: int, H: int, W: int, amp: bool = False):
+    def __init__(self, net, B: int, H: int, W: int, amp: bool = False, det: bool = False):
         from .model.unet import EmbBank, emit_head, emit_stem, emit_time_embed, res_blocks_of
         self.net = net
+        self.det = det
         dev = net._device()
         E, base = net.time_embed_dim, net.base_channel
         shift_blocks = res_blocks_of(net.shift_middle_block, net.shift_output_blocks)
@@ -415,7 +458,7 @@ class ShiftUNetTrainer(_Generation):
         # (fp32-grade) mode -- or, with amp, in the plain "bf16" mode -- with the fused-prologue convs, exactly like sampling;
         # only its skip tensors and bottleneck output are handed to the trainable half.
         self.amp = amp
-        Fp = Plan(dev, "bf16" if amp else "bf16x3")
+        Fp = Plan(dev, "bf16" if amp else "bf16x3", deterministic=det)
         self.x_in = Fp.new((B, net.input_channel, H, W), torch.float32, "x_nchw")
         self.t_in = Fp.new((B,), torch.int64, "t")
         self.x_in.keep = self.t_in.keep = True
@@ -442,7 +485,7 @@ class ShiftUNetTrainer(_Generation):
         emit_head(Fp, net.out, eps_h, self.eps)
         Fp.finalize()
         self.frozen = Fp
-        P = Plan(dev, "fp32")
+        P = Plan(dev, "fp32", deterministic=det)
         P.keep_all = True
         P.train_tc = "bf16" if amp else "bf16x3"   # trainable half: fp32 activations kept, convs on the tensor cores
         self.z_in = P.new((B, net.latent_dim), torch.float32, "z")
@@ -462,7 +505,7 @@ class ShiftUNetTrainer(_Generation):
         self.fwd = P
 
         # ---------------- backward plan ----------------
-        BP = bwd_plan(dev, amp)
+        BP = bwd_plan(dev, amp, det)
         self.sink = GradSink()
         bw = Backward(BP, self.sink)
         self.d_grad = BP.new((B, net.input_channel, H, W), torch.float32, "d_shift_nchw")
@@ -533,11 +576,12 @@ class _ShiftUNetFn(torch.autograd.Function):
 def shiftunet_train_forward(net, x, t, z):
     B, C, H, W = x.shape
     amp = autocast_active()
-    key = ("train", B, H, W, tuple(m.training for m in net._shift_parts()), amp)
+    det = torch.are_deterministic_algorithms_enabled()
+    key = ("train", B, H, W, tuple(m.training for m in net._shift_parts()), amp, det)
     cache = net.__dict__.setdefault("_train_cache", {})
     tr = cache.get(key)
     if tr is None or tr.stale():
-        tr = ShiftUNetTrainer(net, B, H, W, amp)
+        tr = ShiftUNetTrainer(net, B, H, W, amp, det)
         cache[key] = tr
     return _ShiftUNetFn.apply(tr, x, t, z, *tr.params)
 
@@ -546,13 +590,14 @@ def shiftunet_train_forward(net, x, t, z):
 # Plain UNet (regular DPM training, gaussian_diffusion.py:199-211) -- every parameter trainable, skip gradients routed
 # ======================================================================================================================
 class UNetTrainer(_Generation):
-    def __init__(self, net, B: int, H: int, W: int, amp: bool = False):
+    def __init__(self, net, B: int, H: int, W: int, amp: bool = False, det: bool = False):
         from .model.unet import EmbBank, emit_head, res_blocks_of
         from .model.module import timestep_freqs
         self.net = net
         self.amp = amp
+        self.det = det
         dev = net._device()
-        P = Plan(dev, "fp32")
+        P = Plan(dev, "fp32", deterministic=det)
         P.keep_all = True
         P.train_tc = "bf16" if amp else "bf16x3"   # convs on the tensor cores, fp32 activations kept
         E, base, Cimg = net.time_embed_dim, net.base_channel, net.input_channel
@@ -596,7 +641,7 @@ class UNetTrainer(_Generation):
         P.finalize()
         self.fwd = P
 
-        BP = bwd_plan(dev, amp)
+        BP = bwd_plan(dev, amp, det)
         self.sink = GradSink()
         bw = Backward(BP, self.sink)
         self.d_out = BP.new((B, net.output_channel, H, W), torch.float32, "d_eps_nchw")
@@ -632,8 +677,11 @@ class UNetTrainer(_Generation):
         lins = [b.emb_layers[1] for b in blocks]
         d_emb = bw.linear_bank(emb, d_bank, lins, [bank.offsets[id(b)] for b in blocks], bank.total, B=B, E=E, need_dx=True)
         if self.c_in is not None:
-            dwl = BP.new_zeroed(net.label_emb.weight.numel())
-            BP.call("embedding_bwd", d_emb, bw.fx(self.c_in), dwl, B, E, _STREAM)
+            dwl = BP.new_grad(net.label_emb.weight.numel())
+            if det:
+                BP.call("embedding_bwd_det", d_emb, bw.fx(self.c_in), dwl, B, E, net.label_emb.weight.shape[0], _STREAM)
+            else:
+                BP.call("embedding_bwd", d_emb, bw.fx(self.c_in), dwl, B, E, _STREAM)
             self.sink.add(net.label_emb.weight, dwl, net.label_emb.weight.numel(), lambda t: t)
         # emb = Linear2(SiLU(th)) ; th = Linear0(temb)
         d_sth = bw.conv(th, d_emb, te[2].weight, te[2].bias, B=B, H=1, W=1, Cin=E, Cout=E, k=1, a_silu=True,
@@ -682,10 +730,11 @@ def unet_train_forward(net, x, t, cond):
     B, C, H, W = x.shape
     cache = net.__dict__.setdefault("_train_cache", {})
     amp = autocast_active()
-    key = (B, H, W, net.training, amp)
+    det = torch.are_deterministic_algorithms_enabled()
+    key = (B, H, W, net.training, amp, det)
     tr = cache.get(key)
     if tr is None or tr.fwd.stale() or tr.bwd.stale():
-        tr = UNetTrainer(net, B, H, W, amp)
+        tr = UNetTrainer(net, B, H, W, amp, det)
         cache[key] = tr
     return _UNetFn.apply(tr, x, t, cond, *tr.params)
 
@@ -698,11 +747,12 @@ class EncoderTrainer(_Generation):
     plans of a forward under autocast -- its stride-2 and attention convs, their data and weight gradients run as single-pass
     bf16 MMAs (the 3-channel stem and the final Linear stay on CUDA cores)."""
 
-    def __init__(self, enc, B: int, H: int, W: int, amp: bool = False):
+    def __init__(self, enc, B: int, H: int, W: int, amp: bool = False, det: bool = False):
         self.enc = enc
         self.amp = amp
+        self.det = det
         dev = enc._device()
-        P = Plan(dev, "fp32")
+        P = Plan(dev, "fp32", deterministic=det)
         P.keep_all = True
         if amp:
             P.train_tc = "bf16"
@@ -744,7 +794,7 @@ class EncoderTrainer(_Generation):
         P.finalize()
         self.fwd = P
 
-        BP = bwd_plan(dev, amp)
+        BP = bwd_plan(dev, amp, det)
         self.sink = GradSink()
         bw = Backward(BP, self.sink)
         L = enc.latent_dim
@@ -756,18 +806,18 @@ class EncoderTrainer(_Generation):
                 Bc, Hh, Ww, Cc = sv["B"], sv["H"], sv["W"], sv["C"]
                 HW = Hh * Ww
                 K = HW * Cc
-                dw = BP.new_zeroed(K * L)
-                BP.call("conv2d_wgrad_simt", bw.fx(sv["act"]), 0, 0, d, dw, Bc, 1, 1, K, L, 1, 1, 0, _STREAM)
+                dw = BP.new_grad(K * L)
+                bw.wgrad_simt(bw.fx(sv["act"]), 0, 0, d, dw, Bc, 1, 1, K, L, 1, 1, 0)
                 # packed [HW*C][L] (NHWC flatten) -> reference layout [L][C*HW] (NCHW flatten)
                 self.sink.add(m.weight, dw, K * L, lambda t, HW=HW, Cc=Cc: t.view(HW, Cc, L).permute(2, 1, 0))
-                db = BP.new_zeroed(L)
-                BP.call("colsum", d, ctypes.c_int64(Bc), L, db, _STREAM)
+                db = BP.new_grad(L)
+                bw.colsum(d, Bc, L, db)
                 self.sink.add(m.bias, db, L, lambda t: t)
                 wt = m.weight
                 wtco = BP.pack((id(wt), "enc_fc_tco"), [wt],
                                lambda: wt.detach().reshape(L, Cc, HW).permute(0, 2, 1).reshape(L, HW * Cc).float())
                 d_act = BP.new((Bc, Hh, Ww, Cc), torch.float32, "d_fc_in")
-                BP.call("conv2d_dgrad_simt", d, wtco, d_act, Bc, 1, 1, K, L, 1, 1, 0, 0, _STREAM)
+                bw.dgrad_simt(d, wtco, d_act, Bc, 1, 1, K, L, 1, 1, 0)
                 ab, sums, gnm = sv["gn"]
                 d = bw.gn(sv["x"], ab, sums, gnm, d_act, silu=True, resample=RESAMPLE_NONE)
             elif kind == "attn":
@@ -815,10 +865,11 @@ def encoder_train_forward(enc, x):
     B, C, H, W = x.shape
     cache = enc.__dict__.setdefault("_train_cache", {})
     amp = autocast_active()
-    key = (B, H, W, amp)
+    det = torch.are_deterministic_algorithms_enabled()
+    key = (B, H, W, amp, det)
     tr = cache.get(key)
     if tr is None or tr.fwd.stale() or tr.bwd.stale():
-        tr = EncoderTrainer(enc, B, H, W, amp)
+        tr = EncoderTrainer(enc, B, H, W, amp, det)
         cache[key] = tr
     return _EncoderFn.apply(tr, x, *tr.params)
 
@@ -842,7 +893,8 @@ def _tensor_of(b, shape) -> torch.Tensor:
 class MLPTrainer(_Generation):
     """Forward plan keeping every layer's (input, pre-activation, modulation) + backward plan for all parameters of the
     MLPSkipNet; no gradient w.r.t. z_t (the reference's z_t is built from detached latents).  `amp`: the bf16 plans of a
-    forward under autocast (_init_amp)."""
+    forward under autocast (_init_amp).  Its LayerNorm / split-K reductions have no deterministic form yet."""
+    _det_supported = False
 
     def __init__(self, net, B: int, amp: bool = False):
         self.net = net

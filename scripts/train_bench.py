@@ -1,7 +1,7 @@
 """Training-step throughput (SURVEY.md section 8(d) config 5): representation_learning_train_one_batch + backward + gradient
 all-reduce + fused Adam/EMA step on the celeba64-proxy decoder + encoder.
 
-  python scripts/train_bench.py [--batch 32] [--steps 5] [--amp {off,bf16}]               # 1 GPU
+  python scripts/train_bench.py [--batch 32] [--steps 5] [--amp {off,bf16}] [--deterministic {0,1}]   # 1 GPU
   python -m torch.distributed.run --nproc-per-node N ... scripts/train_bench.py --overlap 1   # N GPUs, batch per GPU fixed
 
 Arithmetic: decoder forward, data gradients (conv_tc2) and weight gradients (wgrad_tc) on the tensor cores in the
@@ -11,7 +11,9 @@ plans: frozen half in the "bf16" mode, single-pass bf16 forward convs, data and 
 stride-2 and attention convs (its 3-channel stem and final Linear stay fp32 on CUDA cores).  --overlap 1: the decoder bucket's NCCL all-reduce is launched from a
 post-accumulate-grad hook as soon as the ShiftUNet backward has delivered its gradients and runs while the encoder
 backward computes (pdae_b200.utils.dist.OverlappedGradAllReduce); --overlap 0: all-reduce after backward.
-Rank 0 prints one JSON line."""
+--deterministic 1: the step runs under torch.use_deterministic_algorithms(True, warn_only=True), so the trainers record their
+deterministic plans (no float atomics; bitwise-reproducible on one GPU).  Rank 0 prints one JSON line (with the card's name
+and power limit)."""
 import argparse
 import copy
 import json
@@ -35,7 +37,10 @@ ap.add_argument("--batch", type=int, default=32)
 ap.add_argument("--steps", type=int, default=5)
 ap.add_argument("--overlap", type=int, default=1)
 ap.add_argument("--amp", choices=("off", "bf16"), default="off")
+ap.add_argument("--deterministic", type=int, choices=(0, 1), default=0)
 args = ap.parse_args()
+if args.deterministic:
+    torch.use_deterministic_algorithms(True, warn_only=True)
 world = int(os.environ.get("WORLD_SIZE", "1"))
 rank = int(os.environ.get("RANK", "0"))
 local = int(os.environ.get("LOCAL_RANK", "0"))
@@ -99,7 +104,14 @@ if rank == 0:
            "trainable_params": n_train, "allreduce_bytes_per_step": 4 * n_train if world > 1 else 0,
            "config": "celeba64-proxy encoder + ShiftUNet (shift half trainable), dropout 0.1, fused Adam+EMA; decoder "
                      "forward, data and weight gradients on the tensor cores (split-operand, fp32-grade); encoder "
-                     "and stride-2 / 3-channel convs on CUDA cores (fp32)", "loss": float(loss.detach())}
+                     "and stride-2 / 3-channel convs on CUDA cores (fp32)", "loss": float(loss.detach()),
+           "deterministic": bool(args.deterministic), "gpu": torch.cuda.get_device_name(dev)}
+    try:
+        import subprocess
+        res["power_limit_w"] = subprocess.run(["nvidia-smi", "--query-gpu=power.limit", "--format=csv,noheader,nounits",
+                                               "-i", str(dev.index)], capture_output=True, text=True).stdout.strip()
+    except OSError:
+        pass
     if args.amp != "off":
         res["amp"] = args.amp
         res["config"] = ("celeba64-proxy encoder + ShiftUNet (shift half trainable), dropout 0.1, fused Adam+EMA, bf16 autocast; "
