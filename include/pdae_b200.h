@@ -96,8 +96,9 @@ int pdae_gn_coef_ch(const float* chs1, int C1, const float* chs2, int C2, const 
                     pdae_stream_t stream);
 /* Deterministic forms (torch.use_deterministic_algorithms): bitwise-identical results for identical inputs, no float atomics.
  * Each CTA writes its per-channel partials to its own slot of the caller-owned workspace (no initialisation needed) and the
- * slots are summed in a fixed order; the CTA grid follows (B, HW) only.  workspace: pdae_stats_det_workspace_bytes(B, HW, C)
- * bytes, with C = C1 + C2 for pdae_gn_stats_det (a negative size: bad arguments).  Same outputs and shapes as pdae_ch_stats /
+ * slots are summed in a fixed order; an image's CTAs follow HW only, so its results do not depend on B or on its place in the
+ * batch.  workspace: pdae_stats_det_workspace_bytes(B, HW, C) = B x that of one image, with C = C1 + C2 for pdae_gn_stats_det
+ * (a negative size: bad arguments).  Same outputs and shapes as pdae_ch_stats /
  * pdae_gn_stats (C <= 6144).                                                                                                */
 int64_t pdae_stats_det_workspace_bytes(int B, int HW, int C);
 int pdae_ch_stats_det(const float* src, int B, int HW, int C, float* chs, float* workspace, int64_t workspace_bytes,
@@ -390,7 +391,8 @@ int pdae_conv_tc2_create_splitk(pdae_conv_tc2_plan** plan, const void* in_bf16, 
                                 int B, int Cin, int Cout);
 int pdae_conv_tc2_run(const pdae_conv_tc2_plan* plan, pdae_stream_t stream);
 /* Deterministic plans: switch a forward conv (stride 1 or 2, with or without fused skip), a plain batched GEMM or a split-K
- * Linear plan to the DET kernels (no float atomics).  Statistics as pdae_conv_tc3_set_deterministic.  Split-K: each (tile, k
+ * Linear plan to the DET kernels (no float atomics).  Statistics as pdae_conv_tc3_set_deterministic, a slot per (image, tile)
+ * also when a tile holds several images.  Split-K: each (tile, k
  * range) stores its partial tile in its own slot and the run adds the ranges in order, then the bias, into `out`, which no
  * longer needs zeroing; the number of k ranges follows Cin and Cout only.  Call once, after create and before the first run;
  * workspace: caller-owned, pdae_conv_tc2_det_workspace_bytes(plan) bytes (may be 0).  Other modes: PDAE_EINVAL.              */

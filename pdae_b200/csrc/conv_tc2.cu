@@ -38,11 +38,12 @@
 // item adds its partial tile into the zeroed fp32 output with red.global.add straight from the accumulator fragments
 // (rows past the batch skipped), split 0 adding the bias as well.  fp32 output only: no residual, statistics or bf16 store.
 //
-// DET: the deterministic instantiations (pdae_conv_tc2_set_deterministic) use no float atomics.  Statistics: a tile inside one
-// image stores its per-channel sums in the tile's own slot [B][tiles per image][Cout][2] (plain stores; the run then sums the
-// slots in order); a tile holding several whole images sums each (image, column) with one thread, in row order, straight into
-// [B][Cout][2].  Split-K: item (tile, split) stores its partial tile in slot [split][B][Cout] and the run adds the splits in
-// order, then the bias; the split count follows K and N alone.  The training GEMMs (GM_A_MN / GM_B_MN, the softmax-gradient
+// DET: the deterministic instantiations (pdae_conv_tc2_set_deterministic) use no float atomics.  Statistics: a tile stores
+// each of its images' per-channel sums in the slot [B][tiles per image][Cout][2] of that (image, tile) (plain stores; the run
+// then sums an image's slots in tile order); a tile holding several images sums each (image, column) with one thread, in row
+// order.  With one tile per image the slots are [B][Cout][2] itself.  An image's sums therefore follow its own pixels only,
+// never its batch or its place in a tile.  Split-K: item (tile, split) stores its partial tile in slot [split][B][Cout] and
+// the run adds the splits in order, then the bias; the split count follows K and N alone.  The training GEMMs (GM_A_MN / GM_B_MN, the softmax-gradient
 // epilogue) and the stride-2 data gradient record no statistics, yet their default instantiations still compile the atomic
 // statistics flush; their DET instantiations are the same kernels with that code compiled out.
 #include <cuda.h>
@@ -644,7 +645,9 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
               return x;
             };
             if (DET && p.tn != 1) {
-              // several whole images per tile: (image, column) pairs, each summed over the image's rows in order by one thread
+              // several images per tile: (image, column) pairs, each summed over the image's rows in order by one thread.  When
+              // an image spans several tiles (a grid that is not a power of two, e.g. 6x6 in 2x2 boxes) each tile has its slot.
+              const int tpi = p.tiles_x * p.tiles_y, pimg = ty * p.tiles_x + tx;
               for (int pr = ct; pr < p.tn * CW; pr += T2_CONSUMERS) {
                 const int img = pr / CW, cc = pr - img * CW;
                 if (b0 + img >= p.B) continue;
@@ -663,7 +666,7 @@ conv_tc2_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__
                   sacc += x;
                   qq = fmaf(x, x, qq);
                 }
-                *reinterpret_cast<float2*>(p.ch_stats + ((long long)(b0 + img) * p.Cout + n0 + c * CW + cc) * 2) =
+                *reinterpret_cast<float2*>(p.ch_stats + (((long long)(b0 + img) * tpi + pimg) * p.Cout + n0 + c * CW + cc) * 2) =
                     make_float2(sacc, qq);
               }
             } else if (p.tn == 1) {
@@ -1318,7 +1321,7 @@ extern "C" int64_t pdae_conv_tc2_det_workspace_bytes(const pdae_conv_tc2_plan* p
   const ConvTc2Args& a = pl->args;
   if (pl->gm == GM_SPLITK) return (int64_t)tc2_det_splitk(pl, nullptr) * a.B * a.Cout * (int64_t)sizeof(float);
   const float* stats = pl->det ? pl->det_out : a.ch_stats;
-  if (!stats || a.tn != 1 || a.tiles_x * a.tiles_y == 1) return 0;
+  if (!stats || a.tiles_x * a.tiles_y == 1) return 0;
   return (int64_t)a.B * a.tiles_x * a.tiles_y * a.Cout * 2 * (int64_t)sizeof(float);
 }
 

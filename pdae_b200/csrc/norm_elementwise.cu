@@ -25,6 +25,14 @@ static inline int stats_ppc(int B, int HW) {
   while (ppc > 8 && (long long)B * ((HW + ppc - 1) / ppc) < 592) ppc >>= 1;
   return ppc;
 }
+// pixels per CTA of the deterministic statistics (ch_parts_kernel): from the image size alone, so an image's partial sums are
+// grouped, and added, the same way in every batch.  Halved until one image spans >= 16 CTAs, which keeps a batch of one
+// spread over several SMs at the low-resolution levels (8 pixels at least: 2 CTAs at 4x4, 8 at 8x8, 16 from 16x16 up).
+static inline int stats_ppc_det(int HW) {
+  int ppc = STATS_PIX;
+  while (ppc > 8 && (HW + ppc - 1) / ppc < 16) ppc >>= 1;
+  return ppc;
+}
 
 __global__ void __launch_bounds__(256) gn_stats_kernel(const float* __restrict__ s1, int C1,
                                                        const float* __restrict__ s2, int C2, int HW,
@@ -889,13 +897,13 @@ extern "C" int pdae_gn_coef_ch(const float* chs1, int C1, const float* chs2, int
 }
 
 // Deterministic forms of pdae_ch_stats / pdae_gn_stats: per-CTA partials in the caller's workspace, summed in a fixed order.
-// The CTA count follows (B, HW) only (stats_ppc), so the workspace size does too.
+// An image's CTAs follow HW only (stats_ppc_det), so the workspace is B times one image's slots.
 extern "C" int64_t pdae_stats_det_workspace_bytes(int B, int HW, int C) {
   if (B <= 0 || HW <= 0 || C <= 0) {
     ::pdae::set_error("stats_det_workspace_bytes: B=%d HW=%d C=%d must be > 0", B, HW, C);
     return PDAE_EINVAL;
   }
-  return (int64_t)B * cdiv(HW, stats_ppc(B, HW)) * C * 2 * (int64_t)sizeof(float);
+  return (int64_t)B * cdiv(HW, stats_ppc_det(HW)) * C * 2 * (int64_t)sizeof(float);
 }
 
 static int launch_ch_parts(const char* fn, const float* src1, int C1, const float* src2, int C2, int B, int HW, float* ws,
@@ -903,7 +911,7 @@ static int launch_ch_parts(const char* fn, const float* src1, int C1, const floa
   const int C = C1 + C2;
   PDAE_REQUIRE(B > 0 && HW > 0, "%s: B=%d HW=%d must be > 0", fn, B, HW);
   PDAE_REQUIRE(C1 % 4 == 0 && C2 % 4 == 0 && C > 0 && C <= 6144, "%s: C1=%d C2=%d unsupported", fn, C1, C2);
-  const int ppc = stats_ppc(B, HW), P = cdiv(HW, ppc);
+  const int ppc = stats_ppc_det(HW), P = cdiv(HW, ppc);
   const long long need = (long long)B * P * C * 2 * (long long)sizeof(float);
   PDAE_REQUIRE(ws_bytes >= need, "%s: workspace of %lld bytes, %lld needed (pdae_stats_det_workspace_bytes)", fn,
                (long long)ws_bytes, need);

@@ -42,7 +42,9 @@ def sharded_autoencode(gd, encoder, decoder, x0_all: torch.Tensor, enc_style: st
                        device=None, as_uint8: bool = False) -> torch.Tensor:
     """Autoencode a global batch: every rank runs the hot path on its shard, then one all-gather.
     as_uint8: convert each shard to the reference's wire format first (uint8 NHWC,
-    trainer/train_representation_learning.py:173-174) so the gather moves 4x fewer bytes."""
+    trainer/train_representation_learning.py:173-174) so the gather moves 4x fewer bytes.
+    Under torch.use_deterministic_algorithms(True) the deterministic plans are batch-invariant, so the result is bitwise what
+    one process returns for the whole of x0_all, whatever the world size."""
     world = dist.get_world_size() if dist.is_initialized() else 1
     rank = dist.get_rank() if dist.is_initialized() else 0
     s, e = shard_range(x0_all.shape[0], rank, world)
