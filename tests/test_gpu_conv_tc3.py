@@ -18,7 +18,9 @@ def _p(t):
     return ctypes.c_void_p(t.data_ptr()) if t is not None else None
 
 
-def _run(B, H, W, C1, C2, Cout, x3, out_bf16, res, skip, bn=0, seed=0, silu=1):
+def _run(B, H, W, C1, C2, Cout, x3, out_bf16, res, skip, bn=0, seed=0, silu=1, det=None):
+    """det (optional): det(plan, out, stats) replaces the single pdae_conv_tc3_run (it switches the plan to the deterministic
+    kernel and runs it)."""
     g = torch.Generator(device="cpu").manual_seed(1000 + seed)
     rnd = lambda *s: torch.randn(*s, generator=g)
     Cin = C1 + C2
@@ -51,7 +53,10 @@ def _run(B, H, W, C1, C2, Cout, x3, out_bf16, res, skip, bn=0, seed=0, silu=1):
     _native.check(rc, "pdae_conv_tc3_create")
     try:
         st = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        _native.check(L.pdae_conv_tc3_run(h, st), "pdae_conv_tc3_run")
+        if det is None:
+            _native.check(L.pdae_conv_tc3_run(h, st), "pdae_conv_tc3_run")
+        else:
+            det(h, out, stats)
         torch.cuda.synchronize()
     finally:
         L.pdae_conv_tc3_destroy(h)

@@ -39,11 +39,16 @@ def run_wgrad(B, H, W, Cin, Cout, k, seed=0):
         torch.cuda.synchronize()
     finally:
         L.pdae_wgrad_tc_destroy(h)
-    x = act.double().permute(0, 3, 1, 2)
-    w = torch.zeros(Cout, Cin, k, k, device=DEV, dtype=torch.float64, requires_grad=True)
-    F.conv2d(x, w, padding=k // 2).backward(dy.double().permute(0, 3, 1, 2))
-    ref = w.grad.reshape(Cout, Cin, k * k).permute(2, 1, 0)            # [tap][cin][cout]
-    return dw.double(), ref
+    return dw.double(), wgrad_ref(act.double(), dy.double(), k)
+
+
+def wgrad_ref(act, dy, k, stride=1):
+    """float64 autograd weight gradient of F.conv2d (padding k // 2) in the kernels' layout [tap][cin][cout]; act, dy NHWC."""
+    Cin, Cout = act.shape[3], dy.shape[3]
+    x = act.permute(0, 3, 1, 2)
+    w = torch.zeros(Cout, Cin, k, k, device=act.device, dtype=act.dtype, requires_grad=True)
+    F.conv2d(x, w, stride=stride, padding=k // 2).backward(dy.permute(0, 3, 1, 2))
+    return w.grad.reshape(Cout, Cin, k * k).permute(2, 1, 0)
 
 
 CASES = [
